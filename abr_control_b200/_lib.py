@@ -10,7 +10,8 @@ import threading
 from . import _abi
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# ABRB_LIBRARY: alternative build of the same library (kernel tuning experiments); default is the in-tree build
+# ABRB_LIBRARY: another build of the same library (e.g. of another commit, for an A/B run of bench.py); default is the
+# in-tree build
 LIB_PATH = os.environ.get("ABRB_LIBRARY") or os.path.join(_HERE, "libabrb.so")
 
 _lock = threading.Lock()

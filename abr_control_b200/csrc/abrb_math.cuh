@@ -84,16 +84,12 @@ ABRB_HD void sincos_t(double x, double *s, double *c) { ::sincos(x, s, c); }
 ABRB_HD void sincos_t(float x, float *s, float *c) { ::sincosf(x, s, c); }
 ABRB_HD double sqrt_t(double x) { return ::sqrt(x); }
 ABRB_HD float sqrt_t(float x) { return ::sqrtf(x); }
-// Reciprocal and reciprocal square root of the pivots and norms of the small factorisations.  Default (ABRB_FAST_DIV=1):
-// the hardware seed (rcp / rsqrt.approx.ftz.f64, ~23 bits) refined by two Newton steps to ~1 ulp — the IEEE double
-// division / square root are ~30-instruction dependent sequences each, and these kernels are bound by exactly such
-// chains.  Operands are far from the subnormal range.  ABRB_FAST_DIV=0 keeps the IEEE forms.
-#ifndef ABRB_FAST_DIV
-#define ABRB_FAST_DIV 1
-#endif
+// Reciprocal and reciprocal square root of the pivots and norms of the small factorisations: the hardware seed
+// (rcp / rsqrt.approx.ftz.f64, ~23 bits) refined by two Newton steps to ~1 ulp — the IEEE double division / square root
+// are ~30-instruction dependent sequences each, and these kernels are bound by exactly such chains.  Operands are far
+// from the subnormal range.
 ABRB_HD float inv_t(float x) { return 1.0f / x; }
 ABRB_HD float inv_sqrt_t(float x) { return 1.0f / ::sqrtf(x); }
-#if ABRB_FAST_DIV
 ABRB_HD double inv_t(double x) {
   double r;
 #ifdef __CUDA_ARCH__
@@ -118,16 +114,11 @@ ABRB_HD double inv_sqrt_t(double x) {
   y = ::fma(y, ::fma(-hx * y, y, 0.5), y);
   return ::fma(y, ::fma(-hx * y, y, 0.5), y);
 }
-#else
-ABRB_HD double inv_t(double x) { return 1.0 / x; }
-ABRB_HD double inv_sqrt_t(double x) { return 1.0 / ::sqrt(x); }
-#endif
 // 1 / sqrt(x) to ~2^-45: the hardware seed and ONE Newton step.  Only for the Jacobi rotations of the truncating
 // pseudo-inverse, whose rounds are a pure dependent chain: a rotation whose (c, s) are off by 1e-13 is still applied
 // identically to the row and to its row of V, and the iteration converges to the same decomposition (measured:
 // 5e-13 instead of 4e-14 on the pseudo-inverse, against a 1e-9 parity tolerance; two steps buy nothing there).
 ABRB_HD double inv_sqrt1_t(double x) {
-#if ABRB_FAST_DIV
   double y;
 #ifdef __CUDA_ARCH__
   asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
@@ -136,9 +127,6 @@ ABRB_HD double inv_sqrt1_t(double x) {
   y = (double)(1.0f / ::sqrtf((float)x));
 #endif
   return ::fma(y, ::fma(-0.5 * x * y, y, 0.5), y);
-#else
-  return 1.0 / ::sqrt(x);
-#endif
 }
 ABRB_HD double abs_t(double x) { return ::fabs(x); }
 ABRB_HD float abs_t(float x) { return ::fabsf(x); }
@@ -213,17 +201,8 @@ template <int N, bool ORTHO>
 struct KinSlots {
   static constexpr int kT = 0, kZ = 3 * N, kPl = 6 * N, kR0 = 9 * N, kR1 = 12 * N, kS0 = 15 * N, kS1 = 18 * N;
   // osc_eval parks 1/diag(L), g and C dq in the 3 N link-COM slots at kPl (free by then) while the task-space system is
-  // solved.  ABRB_PARK_L=1 would also park the Cholesky factor of M in N (N + 1) / 2 extra slots at kPark (5.4 KB more
-  // shared memory per warp for UR5 6-DOF fp64); off by default.
-#ifndef ABRB_PARK
-#define ABRB_PARK 1
-#endif
-#ifndef ABRB_PARK_L
-#define ABRB_PARK_L 0
-#endif
-  static constexpr bool kParkL = ABRB_PARK && ABRB_PARK_L && (!ORTHO || N <= 6);
-  static constexpr int kPark = 9 * N;
-  static constexpr int kCount = ORTHO ? 9 * N + (kParkL ? N * (N + 1) / 2 : 0) : 21 * N;
+  // solved.
+  static constexpr int kCount = ORTHO ? 9 * N : 21 * N;
 };
 
 template <typename T, int N, bool ORTHO_, template <typename, int> class Store = RegStore>
@@ -337,8 +316,8 @@ struct Spin {
 // Forward walk along the chain (SURVEY.md Appendix A.1): fills joint origins/axes, link COMs and the
 // full transform of `frame`.
 template <typename T, int N, class K>
-ABRB_HD void walk_unrolled(const ChainK<T, N> &P, const T *q, int frame, K &kin,
-                           T (*link_frames)[12] = nullptr) {  // optional: all link(i+1) frames (rare paths only)
+ABRB_HD void walk(const ChainK<T, N> &P, const T *q, int frame, K &kin,
+                  T (*link_frames)[12] = nullptr) {  // optional: all link(i+1) frames (rare paths only)
   T X[12];
   ABRB_UNROLL
   for (int i = 0; i < 12; ++i) X[i] = P.G0[i];
@@ -404,95 +383,6 @@ ABRB_HD void walk_unrolled(const ChainK<T, N> &P, const T *q, int frame, K &kin,
     ABRB_UNROLL
     for (int j = 0; j < 12; ++j) kin.F[j] = X[j];
   }
-}
-
-// Same walk with the joint loop ROLLED: the body exists once (about 150 instructions instead of 900), the slot
-// indices and the constant-bank offsets become run-time values.  The kernels are instruction-fetch bound (their
-// straight-line code is far larger than the instruction caches, see DESIGN.md S4), so compact loops are worth the
-// few extra address computations.
-template <typename T, int N, class K>
-ABRB_HD void walk_rolled(const ChainK<T, N> &P, const T *q, int frame, K &kin, T (*link_frames)[12] = nullptr) {
-  T X[12];
-  ABRB_UNROLL
-  for (int i = 0; i < 12; ++i) X[i] = P.G0[i];
-  if (frame == 0) {
-    ABRB_UNROLL
-    for (int i = 0; i < 12; ++i) kin.F[i] = P.L0[i];
-  }
-  ABRB_NOUNROLL
-  for (int i = 0; i < N; ++i) {
-    {
-      const T tk[3] = {X[3], X[7], X[11]}, zk[3] = {X[2], X[6], X[10]};
-      kin.st3(K::S::kT + 3 * i, tk);
-      kin.st3(K::S::kZ + 3 * i, zk);
-    }
-    if (!K::kOrtho) {
-      T c0[3], c1[3], c2[3], c12[3], c20[3];
-      ABRB_UNROLL
-      for (int r = 0; r < 3; ++r) {
-        c0[r] = X[r * 4 + 0];
-        c1[r] = X[r * 4 + 1];
-        c2[r] = X[r * 4 + 2];
-      }
-      cross3(c1, c2, c12);
-      cross3(c2, c0, c20);
-      const T inv = T(1) / dot3(c0, c12);
-      ABRB_UNROLL
-      for (int r = 0; r < 3; ++r) {
-        c12[r] *= inv;
-        c20[r] *= inv;
-      }
-      kin.st3(K::S::kR0 + 3 * i, c0);
-      kin.st3(K::S::kR1 + 3 * i, c1);
-      kin.st3(K::S::kS0 + 3 * i, c12);
-      kin.st3(K::S::kS1 + 3 * i, c20);
-    }
-    if (frame == N + 1 + i) {
-      ABRB_UNROLL
-      for (int j = 0; j < 12; ++j) kin.F[j] = X[j];
-    }
-    T qi = q[0];  // q lives in registers: pick q[i] with a select chain instead of a dynamic index
-    ABRB_UNROLL
-    for (int k = 1; k < N; ++k) qi = k == i ? q[k] : qi;
-    T s, c;
-    sincos_t(qi, &s, &c);
-    ABRB_UNROLL
-    for (int r = 0; r < 3; ++r) {
-      const T a = X[r * 4 + 0], b = X[r * 4 + 1];
-      X[r * 4 + 0] = c * a + s * b;
-      X[r * 4 + 1] = c * b - s * a;
-    }
-    const T *Bf = P.Bf[i], *BA = P.BA[i];
-    {
-      T p[3];
-      ABRB_UNROLL
-      for (int r = 0; r < 3; ++r) p[r] = X[r * 4 + 0] * Bf[3] + X[r * 4 + 1] * Bf[7] + X[r * 4 + 2] * Bf[11] + X[r * 4 + 3];
-      kin.st3(K::S::kPl + 3 * i, p);
-    }
-    if (frame == i + 1) aff_mul(X, Bf, kin.F);
-    if (link_frames != nullptr) aff_mul(X, Bf, link_frames[i]);
-    T Y[12];
-    aff_mul(X, BA, Y);
-    ABRB_UNROLL
-    for (int j = 0; j < 12; ++j) X[j] = Y[j];
-  }
-  if (frame == 2 * N + 1) {
-    ABRB_UNROLL
-    for (int j = 0; j < 12; ++j) kin.F[j] = X[j];
-  }
-}
-
-#ifndef ABRB_ROLLED
-#define ABRB_ROLLED 0  // 1: rolled joint/link loops (smaller instruction footprint, more full-width flops;
-                       // tools/kbench.py compares the two), off by default.
-#endif
-
-template <typename T, int N, class K>
-ABRB_HD void walk(const ChainK<T, N> &P, const T *q, int frame, K &kin, T (*link_frames)[12] = nullptr) {
-  if (ABRB_ROLLED)
-    walk_rolled<T, N>(P, q, frame, kin, link_frames);
-  else
-    walk_unrolled<T, N>(P, q, frame, kin, link_frames);
 }
 
 // point `x` of the requested frame in world coordinates  (reference Tx, base_config.py:371-392)
@@ -597,7 +487,7 @@ ABRB_HD void link_columns(const K_ &K, int l, T (*v)[3]) {
   }
 }
 
-// rotational contributions to M, g (and C.dq): shared by the unrolled and the rolled translational loops
+// rotational contributions to M, g (and C.dq)
 template <typename T, int N, bool CDQ, class K_>
 ABRB_HD void dynamics_Mg_rotational(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*M)[N], T *g, T *cdq) {
   constexpr bool ORTHO = K_::kOrtho;
@@ -733,7 +623,7 @@ ABRB_HD void dynamics_C_rotational(const ChainK<T, N> &P, const K_ &K, const T *
 
 // M (upper triangle), g and, if CDQ, the product C.dq
 template <typename T, int N, bool CDQ, class K_>
-ABRB_HD void dynamics_Mg_unrolled(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*M)[N], T *g, T *cdq) {
+ABRB_HD void dynamics_Mg(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*M)[N], T *g, T *cdq) {
   constexpr bool ORTHO = K_::kOrtho;
   ABRB_UNROLL
   for (int a = 0; a < N; ++a) {
@@ -789,7 +679,7 @@ ABRB_HD void dynamics_Mg_unrolled(const ChainK<T, N> &P, const K_ &K, const T *d
 
 // The full Coriolis matrix C (only the rbd kernel materialises it)
 template <typename T, int N, class K_>
-ABRB_HD void dynamics_C_unrolled(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*C)[N]) {
+ABRB_HD void dynamics_C(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*C)[N]) {
   constexpr bool ORTHO = K_::kOrtho;
   ABRB_UNROLL
   for (int a = 0; a < N; ++a)
@@ -824,136 +714,6 @@ ABRB_HD void dynamics_C_unrolled(const ChainK<T, N> &P, const K_ &K, const T *dq
     }
   }
   dynamics_C_rotational<T, N>(P, K, dq, C);
-}
-
-// ---- the same dynamics with the link loop ROLLED (one body, full width): columns of joints k >= l are set to
-// zero so that every accumulation can run unpredicated over all k; more flops than the triangular unrolled form,
-// a fraction of the instruction footprint.
-template <typename T, int N, class K_>
-ABRB_HD void link_columns_masked(const K_ &K, int l, T (*v)[3]) {
-  T pl[3];
-  K.pl(l - 1, pl);  // run-time slot
-  ABRB_UNROLL
-  for (int k = 0; k < N; ++k) {
-    T d[3], tk[3], vk[3];
-    K.t(k, tk);
-    ABRB_UNROLL
-    for (int c = 0; c < 3; ++c) d[c] = pl[c] - tk[c];
-    omega_apply(K, k, d, vk);
-    const bool on = k < l;
-    ABRB_UNROLL
-    for (int c = 0; c < 3; ++c) v[k][c] = on ? vk[c] : T(0);
-  }
-}
-
-template <typename T, int N>
-ABRB_HD T pick(const T *a, int i) {  // a[i] for a register array and a run-time i
-  T r = a[0];
-  ABRB_UNROLL
-  for (int k = 1; k < N; ++k) r = k == i ? a[k] : r;
-  return r;
-}
-
-template <typename T, int N, bool CDQ, class K_>
-ABRB_HD void dynamics_Mg_rolled(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*M)[N], T *g, T *cdq) {
-  constexpr bool ORTHO = K_::kOrtho;
-  ABRB_UNROLL
-  for (int a = 0; a < N; ++a) {
-    g[a] = T(0);
-    if (CDQ) cdq[a] = T(0);
-    ABRB_UNROLL
-    for (int b = 0; b < N; ++b) M[a][b] = T(0);
-  }
-  Spin<T, ORTHO> Wl;
-  Wl.clear();
-  ABRB_NOUNROLL
-  for (int l = 1; l <= N; ++l) {
-    T v[N][3];
-    link_columns_masked<T, N>(K, l, v);
-    const T Wp[3] = {P.Wp[l][0], P.Wp[l][1], P.Wp[l][2]}, gp[3] = {P.gp[l][0], P.gp[l][1], P.gp[l][2]};
-    ABRB_UNROLL
-    for (int b = 0; b < N; ++b) {
-      const T wb[3] = {Wp[0] * v[b][0], Wp[1] * v[b][1], Wp[2] * v[b][2]};
-      g[b] += dot3(v[b], gp);
-      ABRB_UNROLL
-      for (int a = 0; a < N; ++a)
-        if (a <= b) M[a][b] += dot3(v[a], wb);
-    }
-    if (CDQ) {
-      Wl.add(K, l - 1, pick<T, N>(dq, l - 1));
-      Spin<T, ORTHO> tail;
-      tail.clear();
-      T suf[3] = {T(0), T(0), T(0)}, acc[3] = {T(0), T(0), T(0)};
-      ABRB_UNROLL
-      for (int j = N - 1; j >= 0; --j) {
-        const T dqj = j < l ? dq[j] : T(0);  // joints beyond the link contribute nothing
-        tail.add(K, j, dqj);
-        ABRB_UNROLL
-        for (int c = 0; c < 3; ++c) suf[c] += dqj * v[j][c];
-        T a1[3], a2[3];
-        spin_diff_apply(Wl, tail, v[j], a1);
-        omega_apply(K, j, suf, a2);
-        ABRB_UNROLL
-        for (int c = 0; c < 3; ++c) acc[c] += dqj * (a1[c] + a2[c]);
-      }
-      ABRB_UNROLL
-      for (int c = 0; c < 3; ++c) acc[c] *= Wp[c];
-      ABRB_UNROLL
-      for (int k = 0; k < N; ++k) cdq[k] += dot3(v[k], acc);
-    }
-  }
-  dynamics_Mg_rotational<T, N, CDQ>(P, K, dq, M, g, cdq);
-}
-
-template <typename T, int N, class K_>
-ABRB_HD void dynamics_C_rolled(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*C)[N]) {
-  constexpr bool ORTHO = K_::kOrtho;
-  ABRB_UNROLL
-  for (int a = 0; a < N; ++a)
-    ABRB_UNROLL
-  for (int b = 0; b < N; ++b) C[a][b] = T(0);
-  Spin<T, ORTHO> Wl;
-  Wl.clear();
-  ABRB_NOUNROLL
-  for (int l = 1; l <= N; ++l) {
-    T v[N][3];
-    link_columns_masked<T, N>(K, l, v);
-    const T Wp[3] = {P.Wp[l][0], P.Wp[l][1], P.Wp[l][2]};
-    Wl.add(K, l - 1, pick<T, N>(dq, l - 1));
-    Spin<T, ORTHO> tail;
-    tail.clear();
-    T suf[3] = {T(0), T(0), T(0)};
-    ABRB_UNROLL
-    for (int j = N - 1; j >= 0; --j) {
-      const T dqj = j < l ? dq[j] : T(0);
-      tail.add(K, j, dqj);
-      ABRB_UNROLL
-      for (int c = 0; c < 3; ++c) suf[c] += dqj * v[j][c];
-      T a1[3], a2[3], wa[3];
-      spin_diff_apply(Wl, tail, v[j], a1);
-      omega_apply(K, j, suf, a2);
-      ABRB_UNROLL
-      for (int c = 0; c < 3; ++c) wa[c] = Wp[c] * (a1[c] + a2[c]);  // zero for j >= l (v_j = 0, suf = 0)
-      ABRB_UNROLL
-      for (int k = 0; k < N; ++k) C[k][j] += dot3(v[k], wa);
-    }
-  }
-  dynamics_C_rotational<T, N>(P, K, dq, C);
-}
-
-template <typename T, int N, bool CDQ, class K_>
-ABRB_HD void dynamics_Mg(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*M)[N], T *g, T *cdq) {
-  if (ABRB_ROLLED)
-    dynamics_Mg_rolled<T, N, CDQ>(P, K, dq, M, g, cdq);
-  else
-    dynamics_Mg_unrolled<T, N, CDQ>(P, K, dq, M, g, cdq);
-}
-template <typename T, int N, class K_>
-ABRB_HD void dynamics_C(const ChainK<T, N> &P, const K_ &K, const T *dq, T (*C)[N]) {
-  if (ABRB_ROLLED)
-    dynamics_C_rolled<T, N>(P, K, dq, C);
-  else
-    dynamics_C_unrolled<T, N>(P, K, dq, C);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -991,11 +751,7 @@ ABRB_HD void quat_from_R(const T *m, T *qo) {
     T w[4];
     ABRB_UNROLL
     for (int r = 0; r < 4; ++r) w[r] = Kp[r][0] * v[0] + Kp[r][1] * v[1] + Kp[r][2] * v[2] + Kp[r][3] * v[3];
-#if ABRB_FAST_DIV
     const T inv = inv_sqrt_t(w[0] * w[0] + w[1] * w[1] + w[2] * w[2] + w[3] * w[3]);
-#else
-    const T inv = T(1) / sqrt_t(w[0] * w[0] + w[1] * w[1] + w[2] * w[2] + w[3] * w[3]);
-#endif
     ABRB_UNROLL
     for (int r = 0; r < 4; ++r) v[r] = w[r] * inv;
   }
@@ -1149,16 +905,10 @@ ABRB_HD bool chol(T (*A)[S_], T *invd) {  // invd[j] = 1 / L[j][j] (the solves m
     for (int k = 0; k < S_; ++k)
       if (k < j) d -= A[j][k] * A[j][k];
     ok = ok && (d > T(0));
-#if ABRB_FAST_DIV
     const T dpos = d > T(0) ? d : T(1);
     const T inv = inv_sqrt_t(dpos);
     const T ljj = dpos * inv;
     A[j][j] = ljj;
-#else
-    const T ljj = sqrt_t(d > T(0) ? d : T(1));
-    A[j][j] = ljj;
-    const T inv = T(1) / ljj;
-#endif
     invd[j] = inv;
     ABRB_UNROLL
     for (int i = 0; i < S_; ++i) {

@@ -479,18 +479,14 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) K.s.st(Aslot(r, k), row[k]);
   }
-  // ---- nothing below needs L, 1/diag(L), g, C dq, u, u_null until the task-space solve is done: with the scratch in
+  // ---- nothing below needs 1/diag(L), g, C dq until the task-space solve is done: with the scratch in
   //      shared memory they are parked there (slots that are free by now) instead of being carried in registers across
   //      the 6x6 factorisation, where the register allocator would otherwise spill them to local memory
   typedef typename K_::S SL;
-  constexpr bool PARK = K_::kSharedScratch && ABRB_PARK, PARK_L = PARK && SL::kParkL;
+  constexpr bool PARK = K_::kSharedScratch;
   if (PARK) {
-    int li = 0;
     ABRB_UNROLL
     for (int a = 0; a < N; ++a) {
-      ABRB_UNROLL
-      for (int b = 0; b < N; ++b)
-        if (PARK_L && b <= a) K.s.st(SL::kPark + li++, M[a][b]);
       K.s.st(SL::kPl + a, Mi[a]);
       K.s.st(SL::kPl + N + a, g[a]);
       K.s.st(SL::kPl + 2 * N + a, (PLANT || O.use_C) ? cdq[a] : T(0));
@@ -586,15 +582,10 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     wy[k] = sy;
     wz[k] = sz;
   }
-  auto Lget = [&](int a, int b) { return PARK_L ? K.s.ld(SL::kPark + a * (a + 1) / 2 + b) : M[a][b]; };
-  coop.template pinv<T, N, KD>(!fast, K, Lget, y, z, wy, wz, any_null, double(rcond));
+  coop.template pinv<T, N, KD>(!fast, K, [&](int a, int b) { return M[a][b]; }, y, z, wy, wz, any_null, double(rcond));
   if (PARK) {
-    int li = 0;
     ABRB_UNROLL
     for (int a = 0; a < N; ++a) {
-      ABRB_UNROLL
-      for (int b = 0; b < N; ++b)
-        if (PARK_L && b <= a) M[a][b] = K.s.ld(SL::kPark + li++);
       Mi[a] = K.s.ld(SL::kPl + a);
       g[a] = K.s.ld(SL::kPl + N + a);
       cdq[a] = K.s.ld(SL::kPl + 2 * N + a);

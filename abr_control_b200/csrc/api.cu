@@ -55,13 +55,12 @@ int cuda_fail(int e, const char *where) {
   return fail(ABRB_ECUDA, std::string(where) + ": " + cudaGetErrorString((cudaError_t)e));
 }
 
-#ifndef ABRB_N_LIST
-#define ABRB_N_LIST(X) X(1) X(2) X(3) X(4) X(5) X(6) X(7)
-#endif
+// the joint counts kernels.cu is compiled for (Makefile JOINTS)
+#define ABRB_EACH_N(X) X(1) X(2) X(3) X(4) X(5) X(6) X(7)
 
 bool n_supported(int n) {
 #define X(k) if (n == k) return true;
-  ABRB_N_LIST(X)
+  ABRB_EACH_N(X)
 #undef X
   return false;
 }
@@ -327,7 +326,7 @@ static int rbd_eval(const abrb_model *m, int frame_id, const double *x_off, cons
   int e = cudaErrorInvalidValue;
   switch (n) {
 #define X(k) case k: e = launch_rbd<k>(m->host, c); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return e ? cuda_fail(e, "abrb_rbd_eval") : ABRB_OK;
@@ -450,7 +449,7 @@ static int osc_generate(const abrb_osc *c, int frame_id, const double *x_off, co
   int e = cudaErrorInvalidValue;
   switch (n) {
 #define X(j) case j: e = launch_osc<j>(c->model->host, c->params, k); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return e ? cuda_fail(e, "abrb_osc_generate") : ABRB_OK;
@@ -705,8 +704,7 @@ int abrb_gather_wait(abrb_gather *g, void *stream) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  const char *pdl = std::getenv("ABRB_PDL");
-  cfg.numAttrs = (pdl != nullptr && pdl[0] == '0') ? 0 : 1;
+  cfg.numAttrs = 1;
   cudaError_t e = cudaLaunchKernelEx(&cfg, gather_wait_kernel,
                                      (const unsigned long long *)reinterpret_cast<unsigned long long *>(mine + g->flag_off),
                                      g->world, g->epoch, reinterpret_cast<int *>(mine + g->counter_off + 64));
@@ -788,7 +786,7 @@ static int null_generate(const abrb_model *m, const abrb_null_params *p, const v
   int ce = cudaErrorInvalidValue;
   switch (m->host.n) {
 #define X(j) case j: ce = launch_null<j>(m->host, *p, k); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return ce ? cuda_fail(ce, "abrb_null_generate") : ABRB_OK;
@@ -826,7 +824,7 @@ static int sliding_generate(const abrb_model *m, double kd, double lamb, int car
   int e = cudaErrorInvalidValue;
   switch (n) {
 #define X(j) case j: e = launch_sliding<j>(m->host, k); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return e ? cuda_fail(e, "abrb_sliding_generate") : ABRB_OK;
@@ -866,7 +864,7 @@ static int ik_path(const abrb_model *m, double max_dx, double max_dr, double max
   int e = cudaErrorInvalidValue;
   switch (m->host.n) {
 #define X(j) case j: e = launch_ik<j>(m->host, k); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return e ? cuda_fail(e, "abrb_ik_path") : ABRB_OK;
@@ -905,7 +903,7 @@ static int ctrl_generate(const abrb_model *m, int kind, double kp, double kv, in
   int e = cudaErrorInvalidValue;
   switch (n) {
 #define X(j) case j: e = launch_ctrl<j>(m->host, k); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return e ? cuda_fail(e, who) : ABRB_OK;
@@ -957,7 +955,7 @@ static int osc_rollout(const abrb_osc *c, int frame_id, const double *x_off, voi
   int e = cudaErrorInvalidValue;
   switch (n) {
 #define X(j) case j: e = launch_rollout<j>(c->model->host, c->params, k); break;
-    ABRB_N_LIST(X)
+    ABRB_EACH_N(X)
 #undef X
   }
   return e ? cuda_fail(e, "abrb_osc_rollout") : ABRB_OK;

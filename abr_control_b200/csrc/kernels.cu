@@ -6,7 +6,6 @@
 // contiguous per warp; every output array is staged per warp in shared memory and written back with
 // fully coalesced 16-byte stores, so HBM sees whole 128-byte lines only.
 #include <cuda_runtime.h>
-#include <cstdlib>
 #include <utility>
 
 #include <atomic>
@@ -24,21 +23,16 @@ namespace abrb {
 
 namespace {
 
+// CTA size of every kernel.  What ends the OSC kernel is the CTA whose queue of deferred states happens to hold more
+// records than it has groups (a second Jacobi pass); 128 threads give a CTA 20 six-lane groups, 64 would give it half
+// as many per queue.  256 threads do not fit the non-orthonormal fp64 scratch, and for the orthonormal fp64 kernels (54 scratch
+// slots per lane) the evaluation gets slower by about as much as the flush gets cheaper.
 constexpr int kBlock = 128;
-// CTAs per SM the register allocator must allow (tools/kbench.py compares the choices): the fp64 kernels get the full
-// 255 registers (2 CTAs/SM; capping them spills), the fp32 kernels 4 CTAs/SM (128 registers).
-#ifndef ABRB_KSMEM_F32
-#define ABRB_KSMEM_F32 0  // 1: shared-memory kinematic scratch for the fp32 kernels too
-#endif
+// CTAs per SM the register allocator must allow: the fp64 kernels get the full 255 registers (2 CTAs/SM; capping them
+// spills), the fp32 kernels 4 CTAs/SM (128 registers).
 template <typename T>
 struct MinBlocks {
-#ifndef ABRB_MINBLOCKS_F32
-#define ABRB_MINBLOCKS_F32 4
-#endif
-#ifndef ABRB_MINBLOCKS_F64
-#define ABRB_MINBLOCKS_F64 2
-#endif
-  static constexpr int value = sizeof(T) == 8 ? ABRB_MINBLOCKS_F64 : ABRB_MINBLOCKS_F32;
+  static constexpr int value = sizeof(T) == 8 ? 2 : 4;
 };
 constexpr int kWarps = kBlock / 32;
 
@@ -50,21 +44,21 @@ struct MaxRecord {
 
 // Per-warp shared-memory region: holds the warp's kinematic scratch (slot-major, stride 32: lane i owns column i,
 // conflict-free) while a state is being evaluated and is then re-used as the staging tile for the coalesced
-// stores.  KSMEM selects the shared-memory scratch (fp64 kernels: keeps them under the register limit without
-// local-memory spills); otherwise the scratch lives in registers and only the staging tile is needed.
-template <typename T, int N, bool ORTHO, bool KSMEM>
+// stores.  The fp64 kernels keep the scratch in shared memory, which keeps them under the register limit without
+// local-memory spills; the fp32 kernels keep it in registers and need only the staging tile.
+template <typename T, int N, bool ORTHO>
 struct KinSel;
-template <typename T, int N, bool ORTHO>
-struct KinSel<T, N, ORTHO, false> {
-  typedef Kin<T, N, ORTHO, RegStore> type;
+template <int N, bool ORTHO>
+struct KinSel<float, N, ORTHO> {
+  typedef Kin<float, N, ORTHO, RegStore> type;
   static constexpr int kSlots = 0;
-  static __device__ __forceinline__ void bind(type &, T *, int) {}
+  static __device__ __forceinline__ void bind(type &, float *, int) {}
 };
-template <typename T, int N, bool ORTHO>
-struct KinSel<T, N, ORTHO, true> {
-  typedef Kin<T, N, ORTHO, StridedStore> type;
+template <int N, bool ORTHO>
+struct KinSel<double, N, ORTHO> {
+  typedef Kin<double, N, ORTHO, StridedStore> type;
   static constexpr int kSlots = KinSlots<N, ORTHO>::kCount;
-  static __device__ __forceinline__ void bind(type &k, T *warp_region, int lane) {
+  static __device__ __forceinline__ void bind(type &k, double *warp_region, int lane) {
     k.s.base = warp_region + lane;
     k.s.stride = 32;
   }
@@ -132,17 +126,18 @@ struct RbdArgs {
   T xoff[3];
 };
 
-// shared memory per warp: [ kinematic scratch (KSMEM only): kSlots x 32 ][ staging tile: kPitch x max record ]
+// shared memory per warp: [ kinematic scratch (fp64 only): kSlots x 32 ][ staging tile: kPitch x max record ]
 //                        [ exchange area of the cooperative pseudo-inverse (OSC kernels only): XCH x 32 ]
-template <typename T, int N, bool ORTHO, bool KSMEM, int MAXREC, int XCH = 0>
+template <typename T, int N, bool ORTHO, int MAXREC, int XCH = 0>
 struct WarpSmem {
-  static constexpr int kKin = 32 * KinSel<T, N, ORTHO, KSMEM>::kSlots;
+  static constexpr int kKin = 32 * KinSel<T, N, ORTHO>::kSlots;
   static constexpr int kTile = kPitch * (MAXREC < kChunk ? MAXREC : kChunk);
   static constexpr int kXch = 32 * XCH;
   static constexpr int kElems = kKin + kTile + kXch;
 };
-template <typename T, int N, bool ORTHO, int KD, bool KSMEM>
-struct OscSmem : WarpSmem<T, N, ORTHO, KSMEM, (N > 6 ? N : 6), CoopLayout<N, KD, !KSMEM>::kSlots> {};
+template <typename T, int N, bool ORTHO, int KD>
+struct OscSmem : WarpSmem<T, N, ORTHO, (N > 6 ? N : 6),
+                          CoopLayout<N, KD, !KinSel<T, N, ORTHO>::type::kSharedScratch>::kSlots> {};
 
 // Programmatic dependent launch (see launch_pdl): let the stream's next kernel be scheduled as CTAs of this one retire,
 // and wait until the previous kernel of the stream has completed and its memory is visible.  Both are no-ops for a
@@ -152,12 +147,12 @@ __device__ __forceinline__ void pdl_entry() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
-template <typename T, int N, bool ORTHO, bool DYN, bool CMAT, bool XTRA, bool KSMEM>
+template <typename T, int N, bool ORTHO, bool DYN, bool CMAT, bool XTRA>
 __global__ void __launch_bounds__(kBlock, MinBlocks<T>::value)
 rbd_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ RbdArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  typedef KinSel<T, N, ORTHO, KSMEM> KS;
-  typedef WarpSmem<T, N, ORTHO, KSMEM, MaxRecord<N>::value> WS;
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef WarpSmem<T, N, ORTHO, MaxRecord<N>::value> WS;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
   typename KS::type K;
@@ -220,85 +215,42 @@ struct OscQueue {
 // hold one) leave a record in the CTA's queue and are finished by the whole CTA cooperatively (abrb_coop.cuh) once as
 // many as the CTA has groups (20 or 16) have gathered or the CTA has run out of tiles; what does not fit the queue is
 // finished by its warp in line.
-// CTA size of the OSC kernel: 128 threads rather than 64 because what ends the kernel is the CTA whose queue happens to hold more records than it has groups (a second Jacobi pass),
-// and smaller CTAs have fewer groups per queue; 256 threads do not fit the non-orthonormal fp64 scratch.
-#ifndef ABRB_OSC_BLOCK
-#define ABRB_OSC_BLOCK 128
-#endif
-// The orthonormal-chain fp64 kernels (UR5 ...: 54 scratch slots per lane) could afford one 256-thread CTA per SM instead
-// of two 128-thread ones (eight warps sharing the instruction fetches of the same straight-line code, a queue that
-// practically never overflows the CTA's groups), but the evaluation itself gets slower by about as much as the flush
-// gets cheaper, so both stay at 128; the non-orthonormal scratch (126 slots) does not fit eight warps anyway.
-#ifndef ABRB_OSC_BLOCK_ORTHO64
-#define ABRB_OSC_BLOCK_ORTHO64 128
-#endif
-// CTA phase barriers inside the evaluation (abrb_math.cuh, RegStore / StridedStore::sync)
-#ifndef ABRB_OSC_PSYNC_F64
-#define ABRB_OSC_PSYNC_F64 1
-#endif
-#ifndef ABRB_OSC_PSYNC_F32
-#define ABRB_OSC_PSYNC_F32 0
-#endif
-template <typename T>
-struct OscPhaseSync {
-  static constexpr bool value = sizeof(T) == 8 ? (ABRB_OSC_PSYNC_F64 != 0) : (ABRB_OSC_PSYNC_F32 != 0);
-};
-
-template <typename T, bool ORTHO>
-struct OscBlock {
-  static constexpr int value = (ORTHO && sizeof(T) == 8) ? ABRB_OSC_BLOCK_ORTHO64 : ABRB_OSC_BLOCK;
-};
 
 // Resident CTAs per SM the OSC kernel is compiled for.  fp64: 2 (255 registers).  fp32 with orthonormal frames (UR5: the
 // signed-permutation constants fold away): 4 (128 registers) measured best; fp32 with general frames (Jaco2) spills
 // ~3 KB per thread at 128 registers, so it runs 2 CTAs at 255 registers.
-#ifndef ABRB_MINBLOCKS_OSC_F32_GENERAL
-#define ABRB_MINBLOCKS_OSC_F32_GENERAL 2
-#endif
 template <typename T, bool ORTHO>
 struct MinBlocksOsc {
-  static constexpr int value = sizeof(T) == 8 ? MinBlocks<T>::value : (ORTHO ? MinBlocks<T>::value : ABRB_MINBLOCKS_OSC_F32_GENERAL);
+  static constexpr int value = sizeof(T) == 8 || ORTHO ? MinBlocks<T>::value : 2;
 };
 
-template <typename T, int N, bool ORTHO, int KD, bool KSMEM>
-__global__ void __launch_bounds__(OscBlock<T, ORTHO>::value,
-                                  (MinBlocksOsc<T, ORTHO>::value * kBlock / OscBlock<T, ORTHO>::value > 0
-                                       ? MinBlocksOsc<T, ORTHO>::value * kBlock / OscBlock<T, ORTHO>::value : 1))
+template <typename T, int N, bool ORTHO, int KD>
+__global__ void __launch_bounds__(kBlock, MinBlocksOsc<T, ORTHO>::value)
 osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<T, N> O,
            const __grid_constant__ OscArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  typedef KinSel<T, N, ORTHO, KSMEM> KS;
-  typedef OscSmem<T, N, ORTHO, KD, KSMEM> WS;
-  constexpr int kOscBlock = OscBlock<T, ORTHO>::value, kOscWarps = kOscBlock / 32;
-  constexpr int kOscFlushAt = kOscWarps * CoopGroup<N, KD>::kPerWarp;  // one full round of the CTA's groups
-  constexpr int kCoopQueue = kCoopQueuePerWarp * kOscWarps;
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef OscSmem<T, N, ORTHO, KD> WS;
+  constexpr int kOscFlushAt = kWarps * CoopGroup<N, KD>::kPerWarp;  // one full round of the CTA's groups
+  constexpr int kCoopQueue = kCoopQueuePerWarp * kWarps;
   typedef OscQueue<T, N, KD, kCoopQueue> Q;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
   T *stage = region + WS::kKin;
-  unsigned char *qbase = smem_raw + ((size_t)kOscWarps * WS::kElems * sizeof(T) + 15) / 16 * 16;
+  unsigned char *qbase = smem_raw + ((size_t)kWarps * WS::kElems * sizeof(T) + 15) / 16 * 16;
   T *qrec = reinterpret_cast<T *>(qbase);
   long long *qrow = reinterpret_cast<long long *>(qbase + Q::kRowOff);
   int *qcount = reinterpret_cast<int *>(qbase + Q::kCountOff);
   if (threadIdx.x == 0) *qcount = 0;
   __syncthreads();
-#ifdef ABRB_DBG_TIMING  // (timing experiments only) per-CTA cycle counts are written over the training-signal buffer
-  const long long dbg_t0 = clock64();
-  long long dbg_flush = 0, dbg_wait = 0;
-  int dbg_nflush = 0, dbg_rec = 0;
-#endif
   typename KS::type K;
   KS::bind(K, region, lane);
-  K.s.psync = OscPhaseSync<T>::value;
+  K.s.psync = sizeof(T) == 8;  // CTA phase barriers (abrb_math.cuh, RegStore::sync) pay in fp64 only, here and in rollout
   WarpCoop<T, N, KD, typename KS::type> coop{region + WS::kKin + WS::kTile, region, lane, true, qrec, qrow, qcount, 0,
                                              kCoopQueue};
   FlushOut<T> fo;
   fo.u = a.u;
-#ifdef ABRB_DBG_TIMING
-  fo.train = nullptr;
-#else
   fo.train = a.train;
-#endif
   fo.n_peer = a.g.n_peer;
   fo.self = a.g.self;
   fo.row0 = a.g.row0;
@@ -312,10 +264,10 @@ osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<
   pdl_entry();
   // Tiles: the first one is the CTA's own index; the following ones come from the launch's tile counter, so that a CTA
   // whose tiles happen to be expensive (obstacle-active states, many pseudo-inverse states) simply takes fewer of them.
-  const long long n_tiles = (a.B + kOscBlock - 1) / kOscBlock;
+  const long long n_tiles = (a.B + kBlock - 1) / kBlock;
   long long *next_tile = reinterpret_cast<long long *>(qbase + Q::kCountOff + 8);
   for (long long tile = blockIdx.x; tile < n_tiles;) {
-    const int64_t base = tile * kOscBlock;
+    const int64_t base = tile * kBlock;
     // (the next tile's index is asked for now and published at the end of this tile: the atomic's round trip hides
     // under the evaluation)
     long long upcoming = 0;
@@ -343,37 +295,21 @@ osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<
     osc_eval<T, N, KD, false>(P, O, q, dq, tg, a.tv != nullptr ? tv : nullptr, a.ierr != nullptr ? ie : nullptr, u, tr,
                               (T *)nullptr, K, coop);
     if (a.u) store_records<T, N>(a.u, warp_b0, nvalid, u, stage, lane);
-#ifndef ABRB_DBG_TIMING
     if (a.train) store_records<T, N>(a.train, warp_b0, nvalid, tr, stage, lane);
-#endif
     if (a.ierr) store_records<T, 6>(a.ierr, warp_b0, nvalid, ie, stage, lane);
     // fused all-gather: this tile's rows go to every rank's gathered array while the other warps still compute
     for (int p = 0; p < a.g.n_peer; ++p)
       store_records<T, N>(static_cast<T *>(a.g.peer_u[p]), a.g.row0 + warp_b0, nvalid, u, stage, lane);
     // deferred states: emptied once a full round of the CTA's groups has gathered, and after the last tile
-#ifdef ABRB_DBG_TIMING
-    const long long dbg_w0 = clock64();
-#endif
     if (threadIdx.x == 0) *next_tile = upcoming;
     __syncthreads();  // this tile's rows and records, and the next tile's index, are visible to the whole CTA
-#ifdef ABRB_DBG_TIMING
-    dbg_wait += clock64() - dbg_w0;
-    const long long dbg_f0 = clock64();
-#endif
     const int queued = *qcount < kCoopQueue ? *qcount : kCoopQueue;
     tile = *next_tile;
     const bool last = tile >= n_tiles;
     if (queued >= kOscFlushAt || (last && queued > 0)) {
-#ifndef ABRB_DBG_NOFLUSH  // (timing experiments only: results of the deferred states are then wrong)
       coop_flush_cta<T, N, KD>(qrec, qrow, queued, fo, rcond, O.n_null > 0);
-#endif
       __syncthreads();
       if (threadIdx.x == 0) *qcount = 0;
-#ifdef ABRB_DBG_TIMING
-      dbg_flush += clock64() - dbg_f0;
-      dbg_nflush += 1;
-      dbg_rec += queued;
-#endif
     }
     __syncthreads();
   }
@@ -385,17 +321,6 @@ osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<
       __threadfence();
     }
   }
-#ifdef ABRB_DBG_TIMING
-  if (lane == 0 && a.train != nullptr) {
-    T *d = a.train + ((size_t)blockIdx.x * kOscWarps + warp) * 6;
-    d[0] = T(clock64() - dbg_t0);
-    d[1] = T(dbg_flush);
-    d[2] = T(dbg_wait);
-    d[3] = T(dbg_nflush);
-    d[4] = T(dbg_rec);
-    d[5] = T(gridDim.x);
-  }
-#endif
   if (a.g.n_peer > 0) {
     // completion: once every CTA's peer stores are visible system-wide, the last CTA publishes this launch's epoch
     // in every rank's flag array; abrb_gather_wait() on the consumer side spins on those flags
@@ -425,19 +350,19 @@ struct RolloutArgs {
 };
 
 // Closed loop: u = OSC(q, dq); ddq = M^-1 (u + g - C dq); dq += ddq dt; q += dq dt  (state stays in registers)
-template <typename T, int N, bool ORTHO, int KD, bool KSMEM>
+template <typename T, int N, bool ORTHO, int KD>
 __global__ void __launch_bounds__(kBlock)
 rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<T, N> O,
                const __grid_constant__ RolloutArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  typedef KinSel<T, N, ORTHO, KSMEM> KS;
-  typedef OscSmem<T, N, ORTHO, KD, KSMEM> WS;
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef OscSmem<T, N, ORTHO, KD> WS;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
   T *stage = region + WS::kKin;
   typename KS::type K;
   KS::bind(K, region, lane);
-  K.s.psync = OscPhaseSync<T>::value;
+  K.s.psync = sizeof(T) == 8;
   WarpCoop<T, N, KD, typename KS::type> coop{region + WS::kKin + WS::kTile, region, lane, true};
   for (int64_t base = (int64_t)blockIdx.x * kBlock; base < a.B; base += (int64_t)gridDim.x * kBlock) {
     // no early exit (cooperative step inside osc_eval): idle lanes / warps redo a valid state and store nothing
@@ -635,16 +560,6 @@ ik_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ IkArgs
 }
 
 // ------------------------------------------------------------------------------------------------ launch
-// programmatic dependent launch of the OSC kernel (on unless ABRB_PDL=0 in the environment: an A/B switch for timing)
-inline bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char *v = std::getenv("ABRB_PDL");
-    on = (v != nullptr && v[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
-
 // kernel<<<grid, block, smem, stream>>>(args...) with programmatic stream serialization allowed: the launch may be
 // brought onto the SMs while the stream's previous kernel drains; the kernels launched through it (osc_kernel,
 // rbd_kernel) call pdl_entry() before their first global-memory access, which holds them until that kernel has
@@ -661,7 +576,7 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), unsigned grid, unsigned bl
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
@@ -709,9 +624,8 @@ int rbd_go(const ChainHost &h, const RbdCall &c, unsigned want) {
   a.frame = c.frame;
   a.want = want;
   for (int i = 0; i < 3; ++i) a.xoff[i] = c.xoff ? T(c.xoff[i]) : T(0);
-  constexpr bool KSMEM = sizeof(T) == 8 || ABRB_KSMEM_F32 || ABRB_ROLLED;  // rolled loops index the scratch at run time
-  const size_t smem = (size_t)kWarps * WarpSmem<T, N, ORTHO, KSMEM, MaxRecord<N>::value>::kElems * sizeof(T);
-  auto kern = rbd_kernel<T, N, ORTHO, DYN, CMAT, XTRA, KSMEM>;
+  const size_t smem = (size_t)kWarps * WarpSmem<T, N, ORTHO, MaxRecord<N>::value>::kElems * sizeof(T);
+  auto kern = rbd_kernel<T, N, ORTHO, DYN, CMAT, XTRA>;
   cudaError_t e = set_smem(kern, smem);
   if (e != cudaSuccess) return (int)e;
   e = launch_pdl(kern, grid_for(c.B, 8), kBlock, smem, c.stream, P, a);
@@ -765,11 +679,9 @@ int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
   a.tv_stride = c.tv_stride;
   if (c.gather != nullptr) a.g = *c.gather;
   a.sched = c.sched;
-  constexpr bool KSMEM = sizeof(T) == 8 || ABRB_KSMEM_F32 || ABRB_ROLLED;  // rolled loops index the scratch at run time
-  constexpr int kOscBlock = OscBlock<T, ORTHO>::value, kOscWarps = kOscBlock / 32;
-  const size_t smem = ((size_t)kOscWarps * OscSmem<T, N, ORTHO, KD, KSMEM>::kElems * sizeof(T) + 15) / 16 * 16 +
-                      OscQueue<T, N, KD, kCoopQueuePerWarp * kOscWarps>::kBytes;
-  auto kern = osc_kernel<T, N, ORTHO, KD, KSMEM>;
+  const size_t smem = ((size_t)kWarps * OscSmem<T, N, ORTHO, KD>::kElems * sizeof(T) + 15) / 16 * 16 +
+                      OscQueue<T, N, KD, kCoopQueuePerWarp * kWarps>::kBytes;
+  auto kern = osc_kernel<T, N, ORTHO, KD>;
   cudaError_t e = set_smem(kern, smem);
   if (e != cudaSuccess) return (int)e;
   // persistent CTAs: as many as are resident at once, so that each sees several tiles and its deferred states gather
@@ -779,13 +691,13 @@ int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
   cudaGetDevice(&dev);
   if (resident_dev != dev) {
     int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kOscBlock, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kBlock, smem);
     if (e != cudaSuccess) return (int)e;
     resident = per_sm > 0 ? per_sm : 1;
     resident_dev = dev;
   }
-  const int64_t tiles = (c.B + kOscBlock - 1) / kOscBlock, cap = (int64_t)num_sms() * resident;
-  e = launch_pdl(kern, (unsigned)(tiles < cap ? tiles : cap), kOscBlock, smem, c.stream, P, O, a);
+  const int64_t tiles = (c.B + kBlock - 1) / kBlock, cap = (int64_t)num_sms() * resident;
+  e = launch_pdl(kern, (unsigned)(tiles < cap ? tiles : cap), kBlock, smem, c.stream, P, O, a);
   count_launch();
   return e != cudaSuccess ? (int)e : (int)cudaGetLastError();
 }
@@ -808,9 +720,8 @@ int rollout_go(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &
   a.target_stride = c.target_stride;
   a.steps = c.steps;
   a.dt = T(c.dt);
-  constexpr bool KSMEM = sizeof(T) == 8 || ABRB_KSMEM_F32 || ABRB_ROLLED;  // rolled loops index the scratch at run time
-  const size_t smem = (size_t)kWarps * OscSmem<T, N, ORTHO, KD, KSMEM>::kElems * sizeof(T);
-  auto kern = rollout_kernel<T, N, ORTHO, KD, KSMEM>;
+  const size_t smem = (size_t)kWarps * OscSmem<T, N, ORTHO, KD>::kElems * sizeof(T);
+  auto kern = rollout_kernel<T, N, ORTHO, KD>;
   cudaError_t e = set_smem(kern, smem);
   if (e != cudaSuccess) return (int)e;
   kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, O, a);

@@ -1,5 +1,5 @@
 // Micro-benchmark of the warp-cooperative truncating pseudo-inverse (abrb_coop.cuh): cycles per pass, alone on an SM.
-//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 [-DABRB_FAST_DIV=1] -o tools/dbg/coop_time tools/dbg/coop_time.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/dbg/coop_time tools/dbg/coop_time.cu
 //   tools/dbg/coop_time tools/dbg/slow_A.bin     (KD x N = 6 x 6 matrices A of UR5 states on the pinv route, doubles)
 #include <cstdio>
 #include <cstdlib>
