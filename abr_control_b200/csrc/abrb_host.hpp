@@ -164,6 +164,18 @@ inline std::string check_osc(int n, const abrb_osc_params &p) {
   return "";
 }
 
+// Whether an OSC call on an n-joint chain may run the plain instantiation of osc_eval (PLAIN = true, abrb_osc.cuh):
+// plain task-space control of the end effector with gravity and Coriolis compensation.  That is no secondary
+// controller, no target velocity, no integrator (ki == 0, so no integrated-error array), the EE frame, use_g and use_C,
+// and every one of the `kd` task rows the kernel is built for controlled (x, y, z for kd = 3; all six for kd = 6).
+// Everything else runs the general instantiation.
+inline bool osc_plain(const abrb_osc_params &p, int n, int frame, int kd, bool has_tv, bool has_ierr) {
+  if (p.n_null != 0 || has_tv || has_ierr || frame != 2 * n + 1 || !p.use_g || !p.use_C) return false;
+  for (int r = 0; r < 6; ++r)
+    if ((p.ctrlr_dof[r] != 0) != (r < kd)) return false;
+  return true;
+}
+
 template <typename T, int N>
 inline void fill_osc(const abrb_osc_params &p, int frame, const double *x_off, OscK<T, N> &O) {
   O.kp = T(p.kp);

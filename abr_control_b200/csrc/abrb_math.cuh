@@ -163,7 +163,7 @@ ABRB_HD int frame_dep(int frame) {  // number of joints the frame moves with == 
 // Per-state kinematic scratch: joint origins t_k, joint axes z_k, link COMs and (non-orthonormal chains only)
 // columns 0,1 of R_k and rows 0,1 of R_k^-1.  The values live in a "slot store": registers (RegStore) or a strided
 // shared-memory column per thread (StridedStore, slot-major so consecutive lanes hit consecutive words), which is
-// what the fp64 kernels use to stay under the register limit without spilling to local memory.
+// what the fp64 kernels use to keep register pressure, and so local-memory spills, down.
 // Phase barrier of the CTA (`sync()`), called by the per-state code at points every thread of the CTA reaches.  The
 // evaluations are ~10^4 straight-line instructions per state, far beyond the instruction caches, and instruction fetch
 // is their top stall reason; a barrier at the phase boundaries keeps the warps of a CTA inside the same code window so

@@ -272,28 +272,39 @@ struct SeqCoop {
 // `coop`: how the states whose task-space inertia needs the TRUNCATING pseudo-inverse (osc.py:138-145, a few percent
 // of random UR5 states) are finished.  On the GPU every lane of the warp reaches coop.pinv() together and the lanes
 // work on those states jointly (abrb_coop.cuh) instead of one lane walking a long serial path while 31 wait.
-template <typename T, int N, int KD, bool PLANT, class K_, class Coop>
+// PLAIN: the caller has established (osc_plain, abrb_host.hpp) that there is no secondary controller, no target
+// velocity and no integrator, that all KD task rows of the EE frame are controlled, and that use_g and use_C are set.
+// Those branches, their arrays and the per-row mask and per-joint frame selects then vanish at compile time; for the
+// fp64 OSC kernels this is the difference between ~2.5 KB of local-memory spills per thread and none (DESIGN.md S4.1).
+template <typename T, int N, int KD, bool PLANT, bool PLAIN, class K_, class Coop>
 ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, const T *dq, const T *target,
                       const T *tv, T *ierr, T *u, T *train, T *ddq, K_ &K, Coop &coop) {
   constexpr bool ORTHO = K_::kOrtho;
   auto Aslot = [](int r, int k) { return K_::aslot(r, k); };
   T M[N][N], Mi[N], g[N], cdq[N], un[N], y[KD], z[KD];
-  const bool any_null = O.n_null > 0;
+  // (read at each use, as the parameter itself is: a copy would hold a register through the whole evaluation)
+  auto dof_mask = [&]() { return PLAIN ? (1u << KD) - 1u : O.dof_mask; };
+  auto n_null = [&]() { return PLAIN ? 0 : O.n_null; };
+  if (PLAIN) {
+    tv = nullptr;
+    ierr = nullptr;
+  }
+  const bool any_null = n_null() > 0;
   const T rcond = O.thr * T(0.1);
   K.sync();
-  walk<T, N>(P, q, O.frame, K);
+  walk<T, N>(P, q, PLAIN ? 2 * N + 1 : O.frame, K);
   K.sync();
-  const int dep = frame_dep<N>(O.frame);
+  const int dep = frame_dep<N>(PLAIN ? 2 * N + 1 : O.frame);
   T pF[3];
   frame_point(K.F, O.xoff, pF);
 
   // ---- task-space error (osc.py:250-272), needs only the frame
   T err[6] = {T(0), T(0), T(0), T(0), T(0), T(0)};
-  if (O.dof_mask & 7u) {
+  if (dof_mask() & 7u) {
     ABRB_UNROLL
     for (int c = 0; c < 3; ++c) err[c] = pF[c] - target[c];
   }
-  if (KD == 6 && (O.dof_mask & 56u)) {
+  if (KD == 6 && (dof_mask() & 56u)) {
     T R[9];
     ABRB_UNROLL
     for (int r = 0; r < 3; ++r)
@@ -352,7 +363,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
 
   // ---- joint-space dynamics
   K.sync();
-  if (PLANT || O.use_C)
+  if (PLANT || PLAIN || O.use_C)
     dynamics_Mg<T, N, true>(P, K, dq, M, g, cdq);
   else
     dynamics_Mg<T, N, false>(P, K, dq, M, g, nullptr);
@@ -370,7 +381,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     wn[k] = T(0);
     ud[k] = T(0);
   }
-  for (int i = 0; i < O.n_null; ++i) {
+  for (int i = 0; i < n_null(); ++i) {
     const NullK<T, N> &Z = O.nul[i];
     if (Z.kind == kNullDamping) {
       ABRB_UNROLL
@@ -425,7 +436,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     const bool on = k < dep;
     ABRB_UNROLL
     for (int r = 0; r < KD; ++r) {
-      const T val = (on && ((O.dof_mask >> r) & 1u)) ? (r < 3 ? v[r < 3 ? r : 0] : zk[r < 3 ? 0 : r - 3]) : T(0);
+      const T val = (on && ((dof_mask() >> r) & 1u)) ? (r < 3 ? v[r < 3 ? r : 0] : zk[r < 3 ? 0 : r - 3]) : T(0);
       K.s.st(Aslot(r, k), val);
       xdot[r] += val * dq[k];
     }
@@ -435,7 +446,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     for (int r = 0; r < KD; ++r) err[r] += O.kv * (xdot[r] - tv[r]);
   }
   ABRB_UNROLL
-  for (int r = 0; r < KD; ++r) y[r] = ((O.dof_mask >> r) & 1u) ? err[r] : T(0);
+  for (int r = 0; r < KD; ++r) y[r] = ((dof_mask() >> r) & 1u) ? err[r] : T(0);
 
   K.sync();
   // ---- M = L L^T   (osc.py:136)
@@ -454,7 +465,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
       for (int a = 0; a < N; ++a)
         ABRB_UNROLL
       for (int b = 0; b < N; ++b) Lf[a * N + b] = M[a][b];
-      for (int i = 0; i < O.n_null; ++i) {
+      for (int i = 0; i < n_null(); ++i) {
         if (O.nul[i].kind == kNullAvoid) {
           T ua[N], qa[N];  // private copies: only these (not the caller's register arrays) have their address taken
           ABRB_UNROLL
@@ -489,7 +500,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     for (int a = 0; a < N; ++a) {
       K.s.st(SL::kPl + a, Mi[a]);
       K.s.st(SL::kPl + N + a, g[a]);
-      K.s.st(SL::kPl + 2 * N + a, (PLANT || O.use_C) ? cdq[a] : T(0));
+      K.s.st(SL::kPl + 2 * N + a, (PLANT || PLAIN || O.use_C) ? cdq[a] : T(0));
     }
   }
   // ---- S = J M^-1 J^T = A A^T (osc.py:137), built straight into the array that is then factorised in place; z = A w
@@ -502,14 +513,14 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     T za = T(0);
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) za += ra[k] * w[k];
-    z[a] = ((O.dof_mask >> a) & 1u) ? za : T(0);
+    z[a] = (!PLAIN && ((dof_mask() >> a) & 1u)) ? za : T(0);  // (PLAIN: w = 0, and z is read only with any_null)
     ABRB_UNROLL
     for (int b = 0; b < KD; ++b) {
       if (b <= a) {
         T s = T(0);
         ABRB_UNROLL
         for (int k = 0; k < N; ++k) s += ra[k] * K.s.ld(Aslot(b, k));
-        const bool on = ((O.dof_mask >> a) & 1u) && ((O.dof_mask >> b) & 1u);
+        const bool on = ((dof_mask() >> a) & 1u) && ((dof_mask() >> b) & 1u);
         Sc[a][b] = on ? s : (a == b ? T(1) : T(0));
         Sc[b][a] = Sc[a][b];
       }
@@ -529,7 +540,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     T tr = T(0), big = T(0);
     ABRB_UNROLL
     for (int a = 0; a < KD; ++a) {
-      if ((O.dof_mask >> a) & 1u) {
+      if ((dof_mask() >> a) & 1u) {
         T saa = T(0);  // S_aa = sum_k L_ak^2
         ABRB_UNROLL
         for (int b = 0; b < KD; ++b)
@@ -542,7 +553,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
       T fro = T(0);
       ABRB_UNROLL
       for (int a = 0; a < KD; ++a) {
-        if ((O.dof_mask >> a) & 1u) {
+        if ((dof_mask() >> a) & 1u) {
           T e[KD];
           ABRB_UNROLL
           for (int b = 0; b < KD; ++b) e[b] = b == a ? T(1) : T(0);
@@ -608,7 +619,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) u[k] -= jt[k];
   }
-  if (O.use_C) {
+  if (PLAIN || O.use_C) {
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) u[k] -= cdq[k];
   }
@@ -616,7 +627,7 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) train[k] = u[k];  // osc.py:297
   }
-  if (O.use_g) {
+  if (PLAIN || O.use_g) {
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) u[k] -= g[k];
   }
@@ -638,11 +649,11 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
   }
 }
 
-template <typename T, int N, int KD, bool PLANT, class K_>
+template <typename T, int N, int KD, bool PLANT, bool PLAIN = false, class K_>
 ABRB_HD void osc_state(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, const T *dq, const T *target,
                        const T *tv, T *ierr, T *u, T *train, T *ddq, K_ &K) {
   SeqCoop seq;
-  osc_eval<T, N, KD, PLANT>(P, O, q, dq, target, tv, ierr, u, train, ddq, K, seq);
+  osc_eval<T, N, KD, PLANT, PLAIN>(P, O, q, dq, target, tv, ierr, u, train, ddq, K, seq);
 }
 
 // Standalone secondary controller (`Damping/RestingConfig/AvoidObstacles.generate`)

@@ -44,8 +44,8 @@ struct MaxRecord {
 
 // Per-warp shared-memory region: holds the warp's kinematic scratch (slot-major, stride 32: lane i owns column i,
 // conflict-free) while a state is being evaluated and is then re-used as the staging tile for the coalesced
-// stores.  The fp64 kernels keep the scratch in shared memory, which keeps them under the register limit without
-// local-memory spills; the fp32 kernels keep it in registers and need only the staging tile.
+// stores.  The fp64 kernels keep the scratch in shared memory, which is what lets the plain OSC kernels (osc_plain) fit
+// 255 registers without local-memory spills; the fp32 kernels keep it in registers and need only the staging tile.
 template <typename T, int N, bool ORTHO>
 struct KinSel;
 template <int N, bool ORTHO>
@@ -224,7 +224,8 @@ struct MinBlocksOsc {
   static constexpr int value = sizeof(T) == 8 || ORTHO ? MinBlocks<T>::value : 2;
 };
 
-template <typename T, int N, bool ORTHO, int KD>
+// PLAIN: the instantiation for calls that qualify under osc_plain (abrb_host.hpp); see osc_eval.
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
 __global__ void __launch_bounds__(kBlock, MinBlocksOsc<T, ORTHO>::value)
 osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<T, N> O,
            const __grid_constant__ OscArgs<T> a) {
@@ -287,16 +288,16 @@ osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<
 #pragma unroll
     for (int c = 0; c < 6; ++c) {
       tg[c] = a.target[b * a.target_stride + c];
-      tv[c] = a.tv != nullptr ? a.tv[b * a.tv_stride + c] : T(0);
-      ie[c] = a.ierr != nullptr ? a.ierr[b * 6 + c] : T(0);
+      tv[c] = !PLAIN && a.tv != nullptr ? a.tv[b * a.tv_stride + c] : T(0);
+      ie[c] = !PLAIN && a.ierr != nullptr ? a.ierr[b * 6 + c] : T(0);
     }
     coop.valid = lane < nvalid;
     coop.row = b;
-    osc_eval<T, N, KD, false>(P, O, q, dq, tg, a.tv != nullptr ? tv : nullptr, a.ierr != nullptr ? ie : nullptr, u, tr,
+    osc_eval<T, N, KD, false, PLAIN>(P, O, q, dq, tg, a.tv != nullptr ? tv : nullptr, a.ierr != nullptr ? ie : nullptr, u, tr,
                               (T *)nullptr, K, coop);
     if (a.u) store_records<T, N>(a.u, warp_b0, nvalid, u, stage, lane);
     if (a.train) store_records<T, N>(a.train, warp_b0, nvalid, tr, stage, lane);
-    if (a.ierr) store_records<T, 6>(a.ierr, warp_b0, nvalid, ie, stage, lane);
+    if (!PLAIN && a.ierr) store_records<T, 6>(a.ierr, warp_b0, nvalid, ie, stage, lane);
     // fused all-gather: this tile's rows go to every rank's gathered array while the other warps still compute
     for (int p = 0; p < a.g.n_peer; ++p)
       store_records<T, N>(static_cast<T *>(a.g.peer_u[p]), a.g.row0 + warp_b0, nvalid, u, stage, lane);
@@ -307,7 +308,7 @@ osc_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<
     tile = *next_tile;
     const bool last = tile >= n_tiles;
     if (queued >= kOscFlushAt || (last && queued > 0)) {
-      coop_flush_cta<T, N, KD>(qrec, qrow, queued, fo, rcond, O.n_null > 0);
+      coop_flush_cta<T, N, KD>(qrec, qrow, queued, fo, rcond, !PLAIN && O.n_null > 0);
       __syncthreads();
       if (threadIdx.x == 0) *qcount = 0;
     }
@@ -350,7 +351,7 @@ struct RolloutArgs {
 };
 
 // Closed loop: u = OSC(q, dq); ddq = M^-1 (u + g - C dq); dq += ddq dt; q += dq dt  (state stays in registers)
-template <typename T, int N, bool ORTHO, int KD>
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
 __global__ void __launch_bounds__(kBlock)
 rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<T, N> O,
                const __grid_constant__ RolloutArgs<T> a) {
@@ -380,11 +381,11 @@ rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ O
 #pragma unroll
     for (int c = 0; c < 6; ++c) {
       tg[c] = a.target[b * a.target_stride + c];
-      ie[c] = a.ierr != nullptr ? a.ierr[b * 6 + c] : T(0);
+      ie[c] = !PLAIN && a.ierr != nullptr ? a.ierr[b * 6 + c] : T(0);
     }
     coop.valid = lane < nvalid;
     for (int t = 0; t < a.steps; ++t) {
-      osc_eval<T, N, KD, true>(P, O, q, dq, tg, (const T *)nullptr, a.ierr != nullptr ? ie : nullptr, u, (T *)nullptr,
+      osc_eval<T, N, KD, true, PLAIN>(P, O, q, dq, tg, (const T *)nullptr, a.ierr != nullptr ? ie : nullptr, u, (T *)nullptr,
                                acc, K, coop);
 #pragma unroll
       for (int k = 0; k < N; ++k) {
@@ -398,7 +399,7 @@ rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ O
     }
     store_records<T, N>(a.q, warp_b0, nvalid, q, stage, lane);
     store_records<T, N>(a.dq, warp_b0, nvalid, dq, stage, lane);
-    if (a.ierr) store_records<T, 6>(a.ierr, warp_b0, nvalid, ie, stage, lane);
+    if (!PLAIN && a.ierr) store_records<T, 6>(a.ierr, warp_b0, nvalid, ie, stage, lane);
   }
 }
 
@@ -660,8 +661,8 @@ int rbd_dispatch(const ChainHost &h, const RbdCall &c) {
 #undef ABRB_RBD_GO
 }
 
-template <typename T, int N, bool ORTHO, int KD>
-int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
+int osc_launch(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
   ChainK<T, N> P;
   fill_chain<T, N>(h, P);
   OscK<T, N> O;
@@ -681,7 +682,7 @@ int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
   a.sched = c.sched;
   const size_t smem = ((size_t)kWarps * OscSmem<T, N, ORTHO, KD>::kElems * sizeof(T) + 15) / 16 * 16 +
                       OscQueue<T, N, KD, kCoopQueuePerWarp * kWarps>::kBytes;
-  auto kern = osc_kernel<T, N, ORTHO, KD>;
+  auto kern = osc_kernel<T, N, ORTHO, KD, PLAIN>;
   cudaError_t e = set_smem(kern, smem);
   if (e != cudaSuccess) return (int)e;
   // persistent CTAs: as many as are resident at once, so that each sees several tiles and its deferred states gather
@@ -703,7 +704,14 @@ int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
 }
 
 template <typename T, int N, bool ORTHO, int KD>
-int rollout_go(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c) {
+int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
+  // plain task-space control (the headline workload) runs an instantiation without the general kernel's spills
+  if (osc_plain(p, N, c.frame, KD, c.tv != nullptr, c.ierr != nullptr)) return osc_launch<T, N, ORTHO, KD, true>(h, p, c);
+  return osc_launch<T, N, ORTHO, KD, false>(h, p, c);
+}
+
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
+int rollout_launch(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c) {
   ChainK<T, N> P;
   fill_chain<T, N>(h, P);
   OscK<T, N> O;
@@ -721,12 +729,18 @@ int rollout_go(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &
   a.steps = c.steps;
   a.dt = T(c.dt);
   const size_t smem = (size_t)kWarps * OscSmem<T, N, ORTHO, KD>::kElems * sizeof(T);
-  auto kern = rollout_kernel<T, N, ORTHO, KD>;
+  auto kern = rollout_kernel<T, N, ORTHO, KD, PLAIN>;
   cudaError_t e = set_smem(kern, smem);
   if (e != cudaSuccess) return (int)e;
   kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, O, a);
   count_launch();
   return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO, int KD>
+int rollout_go(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c) {
+  if (osc_plain(p, N, c.frame, KD, false, c.ierr != nullptr)) return rollout_launch<T, N, ORTHO, KD, true>(h, p, c);
+  return rollout_launch<T, N, ORTHO, KD, false>(h, p, c);
 }
 
 template <typename T, int N, bool ORTHO>
