@@ -10,7 +10,7 @@
  *   Damping / RestingConfig     controllers/damping.py:21-32, resting_config.py:25-42 + joint.py:104-131
  * numpy.linalg.{inv,det,pinv,eigh} (LAPACK in the reference) are restated as Gauss-Jordan with partial
  * pivoting and cyclic Jacobi; results agree with the NumPy oracle (oracle/osc_oracle.py) to rounding, which
- * tests/test_oracle_c.py checks on the golden cases.
+ * tests/test_oracle_golden.py::test_c_restatement_vs_numpy_oracle checks on the golden cases.
  *
  * The rigid-body quantities J, M, g, C, Tx, R are INPUTS here: either produced by the reference's own
  * generated C (oracle/_ref, see ref_ur5_driver.c — cpu_baseline kind "reference") or by the NumPy oracle.
@@ -343,7 +343,8 @@ void osc_from_quantities(const osc_cfg *c, const double *J6, const double *M, co
   }
 }
 
-/* batch wrapper over precomputed quantities (used by tests/test_oracle_c.py) */
+/* batch wrapper over precomputed quantities (used by tests/test_oracle_golden.py::test_c_restatement_vs_numpy_oracle
+   and tests/test_gpu_fullsize.py) */
 void osc_from_quantities_batch(const osc_cfg *c, long B, const double *J6, const double *M, const double *g,
                                const double *Cm, const double *x, const double *R, const double *q, const double *dq,
                                const double *target, const double *tv, double *u, double *train) {
