@@ -28,6 +28,9 @@ class AbrbError(RuntimeError):
 _VP, _I, _I64, _D, _CP = C.c_void_p, C.c_int, C.c_int64, C.c_double, C.c_char_p
 _gen = [_VP, _I, _VP, _VP, _VP, _VP, _I, _VP, _I, _VP, _VP, _VP, _I64]  # ... u, training_signal, integrated_error, B
 _roll = [_VP, _I, _VP, _VP, _VP, _VP, _I, _I, _D, _VP, _VP, _VP, _VP, _I64, _VP]
+# c, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride, steps, dt, effort_weight,
+# q_traj, dq_traj, u_traj, x_traj, cost, integrated_error, B, stream
+_roll_path = [_VP, _I, _VP, _VP, _VP, _VP, _I, _VP, _I, _I, _D, _D, _VP, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
 SIGNATURES = {
     "abrb_version": (_I, []),
     "abrb_last_error": (_CP, []),
@@ -72,6 +75,8 @@ SIGNATURES = {
     "abrb_ik_path_f32": (_I, [_VP, _D, _D, _D, _I, _D, _I, _VP, _VP, _I, _VP, _VP, _I64, _VP]),
     "abrb_osc_rollout_f64": (_I, _roll),
     "abrb_osc_rollout_f32": (_I, _roll),
+    "abrb_osc_rollout_path_f64": (_I, _roll_path),
+    "abrb_osc_rollout_path_f32": (_I, _roll_path),
     "abrb_launch_count": (_I64, []),
 }
 

@@ -7,6 +7,7 @@ The public names are those of ``abr_control.controllers`` so that a user switche
 name               native entry point (include/abrb.h) / kernel (abr_control_b200/csrc/kernels.cu)
 =================  ==========================================================================================
 OSC                abrb_osc_generate_* / osc_kernel (+ osc_finish_kernel in the two-launch mode), rollout_kernel
+OSC.rollout_path   abrb_osc_rollout_path_* / rollout_kernel with per-step targets (RolloutPathArgs)
 Damping            secondary-controller kind 1: fused into osc_kernel, or abrb_null_generate_* / null_kernel
 RestingConfig      secondary-controller kind 2 (same two routes)
 AvoidObstacles     secondary-controller kind 3 (same two routes)

@@ -336,6 +336,87 @@ class OSC(Controller):
             return qa[0], dqa[0], {k: v[:, 0] for k, v in traj.items()}
         return qa, dqa, traj
 
+    def rollout_path(self, q, dq, path, dt=1e-3, path_velocity=None, ref_frame="EE", xyz_offset=None,
+                     record=("q", "dq", "u", "x"), effort_weight=0.0):
+        """Path-following closed-loop rollout on the GPU (include/abrb.h, abrb_osc_rollout_path_*): for each step
+        ``t = 0 .. S-1``::
+
+            x_t = Tx(ref_frame, q_t, x=xyz_offset)
+            u_t = generate(q_t, dq_t, target=path[t], target_velocity=path_velocity[t])
+            ddq = M^-1 (u_t + g - C dq_t);  dq_{t+1} = dq_t + ddq dt;  q_{t+1} = q_t + dq_{t+1} dt
+            cost += |x_t - path[t, :3]|^2 + effort_weight * |u_t|^2
+
+        ``path`` and ``path_velocity`` are ``(S, 6)`` (one path shared by every trajectory) or ``(S, B, 6)`` (one per
+        trajectory); each row is (x, y, z, Euler a, b, g) like ``generate``'s target.  A velocity row that is all zero
+        (or no ``path_velocity``) gives ``generate``'s -kv M dq damping.  From a reference ``PathPlanner`` result
+        ``P = planner.generate_path(...)`` (rows: position, velocity, orientation, angular velocity)::
+
+            path = np.hstack([P[:, :3], P[:, 6:9]]);  path_velocity = np.hstack([P[:, 3:6], P[:, 9:12]])
+
+        Returns ``(q_final, dq_final, traj, cost)``: ``traj[k]`` for k in ``record`` is ``(S, B, n)`` (``"x"``:
+        ``(S, B, 3)``), ``cost`` is ``(B,)``.  ``traj["x"][t]`` and ``traj["u"][t]`` belong to the state before step t,
+        ``traj["q"][t]`` and ``traj["dq"][t]`` to the state after it (as in ``rollout``).  ``record=()`` returns only the
+        final state and the cost: the allocation-light form for sampling-based MPC.  CUDA tensors in -> CUDA tensors
+        out; NumPy in -> NumPy out; a single state ``q`` of shape ``(n,)`` takes an ``(S, 6)`` path and returns
+        ``(S, n)`` records and a scalar cost.  With ``ki != 0`` the rollout starts from the controller's integrator
+        state and leaves it updated, as ``rollout`` does.
+        """
+        import torch
+
+        rc = self.robot_config
+        qa, dqa, single, kind, f32 = _batch.prep_state(rc, q, dq)
+        if kind == "numpy":
+            dev = torch.device("cuda", torch.cuda.current_device())
+            qa, dqa = torch.as_tensor(qa).to(dev), torch.as_tensor(dqa).to(dev)
+        else:
+            qa, dqa = qa.clone(), dqa.clone()
+        B, n = qa.shape
+
+        def rows(x, what):
+            t = x if _batch.is_torch(x) else torch.as_tensor(np.asarray(x, dtype=np.float64))
+            t = t.to(device=qa.device, dtype=qa.dtype).contiguous()
+            if t.dim() == 2 and t.shape[1] == 6:
+                return t, 0
+            if t.dim() == 3 and t.shape[1:] == (B, 6):
+                return t, 6
+            raise ValueError(f"{what} must have shape (S, 6) or (S, {B}, 6)")
+
+        pth, pstride = rows(path, "path")
+        steps = pth.shape[0]
+        pv, pvstride = (None, 0)
+        if path_velocity is not None:
+            pv, pvstride = rows(path_velocity, "path_velocity")
+            if pv.shape[0] != steps:
+                raise ValueError(f"path_velocity has {pv.shape[0]} steps, path has {steps}")
+        fid = rc.frame_id(ref_frame)
+        xo = None
+        if xyz_offset is not None and not np.allclose(np.asarray(xyz_offset, dtype=float), 0):
+            xo = (C.c_double * 3)(*[float(v) for v in np.asarray(xyz_offset, dtype=float).reshape(3)])
+        for k in record:
+            if k not in ("q", "dq", "u", "x"):
+                raise ValueError(f"rollout_path can record 'q', 'dq', 'u' and 'x', not {k!r}")
+        traj = {k: torch.empty((steps, B, 3 if k == "x" else n), dtype=qa.dtype, device=qa.device) for k in record}
+        cost = torch.empty((B,), dtype=qa.dtype, device=qa.device)
+        ie = None
+        if self.ki != 0:
+            ie = self._ierr_for(qa, "torch", single)
+        L = _lib.lib()
+        fn = L.abrb_osc_rollout_path_f32 if f32 else L.abrb_osc_rollout_path_f64
+        with torch.cuda.device(qa.device):
+            _lib.check(fn(self._native(), fid, xo, qa.data_ptr(), dqa.data_ptr(), pth.data_ptr(), pstride,
+                          _batch.ptr(pv), pvstride, int(steps), float(dt), float(effort_weight),
+                          _batch.ptr(traj.get("q")), _batch.ptr(traj.get("dq")), _batch.ptr(traj.get("u")),
+                          _batch.ptr(traj.get("x")), cost.data_ptr(), _batch.ptr(ie), B,
+                          torch.cuda.current_stream(qa.device).cuda_stream))
+        if ie is not None and single:
+            self.integrated_error = ie[0].double().cpu().numpy()
+        if kind == "numpy":
+            qa, dqa, cost = qa.cpu().numpy(), dqa.cpu().numpy(), cost.cpu().numpy()
+            traj = {k: v.cpu().numpy() for k, v in traj.items()}
+        if single:
+            return qa[0], dqa[0], {k: v[:, 0] for k, v in traj.items()}, cost[0]
+        return qa, dqa, traj, cost
+
 
 class _Pending:
     """Result of ``OSC.generate_async``: ``wait()`` blocks until the batch has left the GPU and returns ``u``."""

@@ -58,6 +58,15 @@ struct RolloutCall {
   void *ierr = nullptr;  // (B, 6) integrated task-space error, in/out (device), only with ki != 0
 };
 
+// abrb_osc_rollout_path_*: `target` / `target_stride` hold the path, (steps, B, 6) for stride 6, (steps, 6) for 0
+struct RolloutPathCall : RolloutCall {
+  const void *tv = nullptr;  // path velocity, laid out like the path per tv_stride, or nullptr
+  int tv_stride = 0;
+  void *x_traj = nullptr;    // (steps, B, 3) or nullptr
+  void *cost = nullptr;      // (B,) or nullptr
+  double effort_weight = 0;
+};
+
 struct NullCall {
   const void *q, *dq;
   void *u;
@@ -106,6 +115,7 @@ struct IkCall {
 template <int N> int launch_rbd(const ChainHost &h, const RbdCall &c);
 template <int N> int launch_osc(const ChainHost &h, const abrb_osc_params &p, const OscCall &c);
 template <int N> int launch_rollout(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c);
+template <int N> int launch_rollout_path(const ChainHost &h, const abrb_osc_params &p, const RolloutPathCall &c);
 template <int N> int launch_null(const ChainHost &h, const abrb_null_params &z, const NullCall &c);
 template <int N> int launch_ctrl(const ChainHost &h, const CtrlCall &c);
 template <int N> int launch_sliding(const ChainHost &h, const SlidingCall &c);

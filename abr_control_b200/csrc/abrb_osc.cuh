@@ -276,9 +276,10 @@ struct SeqCoop {
 // velocity and no integrator, that all KD task rows of the EE frame are controlled, and that use_g and use_C are set.
 // Those branches, their arrays and the per-row mask and per-joint frame selects then vanish at compile time; for the
 // fp64 OSC kernels this is the difference between ~2.5 KB of local-memory spills per thread and none (DESIGN.md S4.1).
+// `x`: receives the control point (ref_frame + xyz_offset) at q, 3 values, or nullptr.
 template <typename T, int N, int KD, bool PLANT, bool PLAIN, class K_, class Coop>
 ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, const T *dq, const T *target,
-                      const T *tv, T *ierr, T *u, T *train, T *ddq, K_ &K, Coop &coop) {
+                      const T *tv, T *ierr, T *u, T *train, T *ddq, K_ &K, Coop &coop, T *x = nullptr) {
   constexpr bool ORTHO = K_::kOrtho;
   auto Aslot = [](int r, int k) { return K_::aslot(r, k); };
   T M[N][N], Mi[N], g[N], cdq[N], un[N], y[KD], z[KD];
@@ -297,6 +298,10 @@ ABRB_HD void osc_eval(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, co
   const int dep = frame_dep<N>(PLAIN ? 2 * N + 1 : O.frame);
   T pF[3];
   frame_point(K.F, O.xoff, pF);
+  if (x != nullptr) {
+    ABRB_UNROLL
+    for (int c = 0; c < 3; ++c) x[c] = pF[c];
+  }
 
   // ---- task-space error (osc.py:250-272), needs only the frame
   T err[6] = {T(0), T(0), T(0), T(0), T(0), T(0)};
@@ -654,6 +659,40 @@ ABRB_HD void osc_state(const ChainK<T, N> &P, const OscK<T, N> &O, const T *q, c
                        const T *tv, T *ierr, T *u, T *train, T *ddq, K_ &K) {
   SeqCoop seq;
   osc_eval<T, N, KD, PLANT, PLAIN>(P, O, q, dq, target, tv, ierr, u, train, ddq, K, seq);
+}
+
+// Row t of trajectory b of a path (or path velocity) of abrb_osc_rollout_path_*: (steps, B, 6) when stride == 6, one
+// (steps, 6) path for every trajectory when stride == 0.
+template <typename T>
+ABRB_HD const T *path_row(const T *path, int stride, int t, int64_t B, int64_t b) {
+  return path + (stride != 0 ? ((int64_t)t * B + b) * 6 : (int64_t)t * 6);
+}
+
+// One step of the closed-loop rollouts (rollout_kernel, fixed target and path):
+//     u = OSC(q, dq, target, tv);  ddq = M^-1 (u + g - C dq);  dq += ddq dt;  q += dq dt
+// (semi-implicit Euler).  PATH: also `x` = the control point at the state BEFORE the update, and
+//     cost += |x - target[:3]|^2 + effort |u|^2.
+template <typename T, int N, int KD, bool PLAIN, bool PATH, class K_, class Coop>
+ABRB_HD void rollout_step(const ChainK<T, N> &P, const OscK<T, N> &O, T *q, T *dq, const T *target, const T *tv,
+                          T *ierr, T dt, T effort, T *u, T *x, T &cost, K_ &K, Coop &coop) {
+  T acc[N];
+  osc_eval<T, N, KD, true, PLAIN>(P, O, q, dq, target, tv, ierr, u, (T *)nullptr, acc, K, coop, PATH ? x : (T *)nullptr);
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) {
+    dq[k] += acc[k] * dt;
+    q[k] += dq[k] * dt;
+  }
+  if (PATH) {
+    T ex = T(0), eu = T(0);
+    ABRB_UNROLL
+    for (int c = 0; c < 3; ++c) {
+      const T d = x[c] - target[c];
+      ex += d * d;
+    }
+    ABRB_UNROLL
+    for (int k = 0; k < N; ++k) eu += u[k] * u[k];
+    cost += ex + effort * eu;
+  }
 }
 
 // Standalone secondary controller (`Damping/RestingConfig/AvoidObstacles.generate`)

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -972,6 +973,86 @@ int abrb_osc_rollout_f32(const abrb_osc *c, int frame_id, const double *x_off, f
                          float *integrated_error, int64_t B, void *stream) {
   return osc_rollout(c, frame_id, x_off, q, dq, target, target_stride, steps, dt, q_traj, dq_traj, u_traj,
                      integrated_error, B, stream, true);
+}
+
+// ------------------------------------------------------------------------------------------------ path rollout
+static int osc_rollout_path(const abrb_osc *c, int frame_id, const double *x_off, void *q, void *dq, const void *path,
+                            int path_stride, const void *path_velocity, int pv_stride, int steps, double dt,
+                            double effort_weight, void *q_traj, void *dq_traj, void *u_traj, void *x_traj, void *cost,
+                            void *ierr, int64_t B, void *stream, bool f32) {
+  const char *who = "abrb_osc_rollout_path";
+  const std::string w(who);
+  if (!c) return fail(ABRB_EINVAL, w + ": NULL controller");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (steps < 0) return fail(ABRB_EINVAL, w + ": steps < 0");
+  const int n = c->model->host.n;
+  if (frame_id < 0 || frame_id > 2 * n + 1) return fail(ABRB_EFRAME, w + ": invalid frame id");
+  if (path_stride != 0 && path_stride != 6) return fail(ABRB_EINVAL, w + ": path_stride must be 0 or 6");
+  if (pv_stride != 0 && pv_stride != 6) return fail(ABRB_EINVAL, w + ": pv_stride must be 0 or 6");
+  if (!std::isfinite(effort_weight) || effort_weight < 0.0)
+    return fail(ABRB_EINVAL, w + ": effort_weight must be finite and >= 0");
+  if ((c->params.ki != 0.0) != (ierr != nullptr))
+    return fail(ABRB_EINVAL, w + ": integrated_error must be given if and only if ki != 0");
+  if (B == 0) return ABRB_OK;
+  if (!q) return fail(ABRB_EINVAL, w + ": NULL q");
+  if (!dq) return fail(ABRB_EINVAL, w + ": NULL dq");
+  if (steps > 0 && !path) return fail(ABRB_EINVAL, w + ": NULL path");
+  const void *ptrs[] = {q, dq, path, path_velocity, q_traj, dq_traj, u_traj, x_traj, cost, ierr};
+  const char *names[] = {"q", "dq", "path", "path_velocity", "q_traj", "dq_traj", "u_traj", "x_traj", "cost",
+                         "integrated_error"};
+  for (int i = 0; i < 10; ++i)
+    if (ptrs[i] && !aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  if (steps == 0) {  // nothing to step: q, dq and the integrator stay as they are, the cost is zero
+    int e = cost ? (int)cudaMemsetAsync(cost, 0, (size_t)B * (f32 ? 4 : 8), (cudaStream_t)stream) : 0;
+    return e ? cuda_fail(e, who) : ABRB_OK;
+  }
+  RolloutPathCall k;
+  k.frame = frame_id;
+  k.xoff = x_off;
+  k.q = q;
+  k.dq = dq;
+  k.target = path;
+  k.target_stride = path_stride;
+  k.steps = steps;
+  k.dt = dt;
+  k.q_traj = q_traj;
+  k.dq_traj = dq_traj;
+  k.u_traj = u_traj;
+  k.B = B;
+  k.f32 = f32;
+  k.stream = (cudaStream_t)stream;
+  k.ierr = ierr;
+  k.tv = path_velocity;
+  k.tv_stride = pv_stride;
+  k.x_traj = x_traj;
+  k.cost = cost;
+  k.effort_weight = effort_weight;
+  int e = cudaErrorInvalidValue;
+  switch (n) {
+#define X(j) case j: e = launch_rollout_path<j>(c->model->host, c->params, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_osc_rollout_path_f64(const abrb_osc *c, int frame_id, const double *x_off, double *q, double *dq,
+                              const double *path, int path_stride, const double *path_velocity, int pv_stride,
+                              int steps, double dt, double effort_weight, double *q_traj, double *dq_traj,
+                              double *u_traj, double *x_traj, double *cost, double *integrated_error, int64_t B,
+                              void *stream) {
+  return osc_rollout_path(c, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride, steps, dt,
+                          effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, integrated_error, B, stream, false);
+}
+int abrb_osc_rollout_path_f32(const abrb_osc *c, int frame_id, const double *x_off, float *q, float *dq,
+                              const float *path, int path_stride, const float *path_velocity, int pv_stride,
+                              int steps, double dt, double effort_weight, float *q_traj, float *dq_traj,
+                              float *u_traj, float *x_traj, float *cost, float *integrated_error, int64_t B,
+                              void *stream) {
+  return osc_rollout_path(c, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride, steps, dt,
+                          effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, integrated_error, B, stream, true);
 }
 
 }  // extern "C"

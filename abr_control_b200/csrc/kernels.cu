@@ -6,6 +6,7 @@
 // contiguous per warp; every output array is staged per warp in shared memory and written back with
 // fully coalesced 16-byte stores, so HBM sees whole 128-byte lines only.
 #include <cuda_runtime.h>
+#include <type_traits>
 #include <utility>
 
 #include <atomic>
@@ -350,11 +351,26 @@ struct RolloutArgs {
   T dt;
 };
 
-// Closed loop: u = OSC(q, dq); ddq = M^-1 (u + g - C dq); dq += ddq dt; q += dq dt  (state stays in registers)
-template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
+// Path-following rollout: `target` is the path, element (t, b, c) at target[(t B + b) 6 + c] when target_stride == 6
+// (one path per trajectory) or at target[t 6 + c] when 0 (one path shared by every trajectory); `tv` likewise.
+template <typename T>
+struct RolloutPathArgs : RolloutArgs<T> {
+  const T *tv;       // path velocity, or nullptr
+  T *x_traj, *cost;  // (steps, B, 3) control-point track, (B,) tracking cost, or nullptr
+  int tv_stride;
+  T effort;          // weight of |u|^2 in the cost
+};
+
+// Closed loop: u = OSC(q, dq); ddq = M^-1 (u + g - C dq); dq += ddq dt; q += dq dt  (state stays in registers).
+// Args = RolloutArgs: one fixed target per trajectory (abrb_osc_rollout_*).  Args = RolloutPathArgs: the target and
+// target velocity of step t come from the path, and the control point of each step's state and the tracking cost are
+// recorded too (abrb_osc_rollout_path_*).  (The two share this body as one kernel template: moving the loop into a
+// device function of its own changes the generated code of the fixed-target instantiations.)
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN, class Args>
 __global__ void __launch_bounds__(kBlock)
 rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ OscK<T, N> O,
-               const __grid_constant__ RolloutArgs<T> a) {
+               const __grid_constant__ Args a) {
+  constexpr bool PATH = std::is_same<Args, RolloutPathArgs<T>>::value;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   typedef KinSel<T, N, ORTHO> KS;
   typedef OscSmem<T, N, ORTHO, KD> WS;
@@ -372,7 +388,8 @@ rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ O
     const int nvalid = rem < 32 ? (rem > 0 ? (int)rem : 0) : 32;
     const int64_t bb = warp_b0 + (lane < nvalid ? lane : nvalid - 1);
     const int64_t b = bb < a.B ? (bb >= 0 ? bb : 0) : a.B - 1;
-    T q[N], dq[N], tg[6], ie[6], u[N], acc[N];
+    T q[N], dq[N], tg[6], ie[6], u[N], tv[6], x[3];
+    T cost = T(0);
 #pragma unroll
     for (int k = 0; k < N; ++k) {
       q[k] = a.q[b * N + k];
@@ -380,26 +397,42 @@ rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ O
     }
 #pragma unroll
     for (int c = 0; c < 6; ++c) {
-      tg[c] = a.target[b * a.target_stride + c];
+      if (!PATH) tg[c] = a.target[b * a.target_stride + c];
       ie[c] = !PLAIN && a.ierr != nullptr ? a.ierr[b * 6 + c] : T(0);
     }
     coop.valid = lane < nvalid;
     for (int t = 0; t < a.steps; ++t) {
-      osc_eval<T, N, KD, true, PLAIN>(P, O, q, dq, tg, (const T *)nullptr, a.ierr != nullptr ? ie : nullptr, u, (T *)nullptr,
-                               acc, K, coop);
+      const T *tvp = nullptr;
+      T effort = T(0);
+      if constexpr (PATH) {
+        // a shared path is one address for the whole warp (a broadcast load); a per-trajectory path is one row per lane
+        const T *pt = path_row(a.target, a.target_stride, t, a.B, b);
 #pragma unroll
-      for (int k = 0; k < N; ++k) {
-        dq[k] += acc[k] * a.dt;
-        q[k] += dq[k] * a.dt;
+        for (int c = 0; c < 6; ++c) tg[c] = pt[c];
+        if (!PLAIN && a.tv != nullptr) {
+          const T *vt = path_row(a.tv, a.tv_stride, t, a.B, b);
+#pragma unroll
+          for (int c = 0; c < 6; ++c) tv[c] = vt[c];
+          tvp = tv;
+        }
+        effort = a.effort;
       }
+      rollout_step<T, N, KD, PLAIN, PATH>(P, O, q, dq, tg, tvp, a.ierr != nullptr ? ie : nullptr, a.dt, effort, u, x,
+                                          cost, K, coop);
       const int64_t row0 = (int64_t)t * a.B + warp_b0;
       if (a.u_traj) store_records<T, N>(a.u_traj, row0, nvalid, u, stage, lane);
       if (a.q_traj) store_records<T, N>(a.q_traj, row0, nvalid, q, stage, lane);
       if (a.dq_traj) store_records<T, N>(a.dq_traj, row0, nvalid, dq, stage, lane);
+      if constexpr (PATH) {
+        if (a.x_traj) store_records<T, 3>(a.x_traj, row0, nvalid, x, stage, lane);
+      }
     }
     store_records<T, N>(a.q, warp_b0, nvalid, q, stage, lane);
     store_records<T, N>(a.dq, warp_b0, nvalid, dq, stage, lane);
     if (!PLAIN && a.ierr) store_records<T, 6>(a.ierr, warp_b0, nvalid, ie, stage, lane);
+    if constexpr (PATH) {
+      if (a.cost != nullptr && lane < nvalid) a.cost[b] = cost;
+    }
   }
 }
 
@@ -710,13 +743,8 @@ int osc_go(const ChainHost &h, const abrb_osc_params &p, const OscCall &c) {
   return osc_launch<T, N, ORTHO, KD, false>(h, p, c);
 }
 
-template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
-int rollout_launch(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c) {
-  ChainK<T, N> P;
-  fill_chain<T, N>(h, P);
-  OscK<T, N> O;
-  fill_osc<T, N>(p, c.frame, c.xoff, O);
-  RolloutArgs<T> a;
+template <typename T>
+void fill_rollout_args(const RolloutCall &c, RolloutArgs<T> &a) {
   a.q = static_cast<T *>(c.q);
   a.dq = static_cast<T *>(c.dq);
   a.target = static_cast<const T *>(c.target);
@@ -728,8 +756,48 @@ int rollout_launch(const ChainHost &h, const abrb_osc_params &p, const RolloutCa
   a.target_stride = c.target_stride;
   a.steps = c.steps;
   a.dt = T(c.dt);
+}
+
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
+int rollout_path_launch(const ChainHost &h, const abrb_osc_params &p, const RolloutPathCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  OscK<T, N> O;
+  fill_osc<T, N>(p, c.frame, c.xoff, O);
+  RolloutPathArgs<T> a;
+  fill_rollout_args<T>(c, a);
+  a.tv = static_cast<const T *>(c.tv);
+  a.x_traj = static_cast<T *>(c.x_traj);
+  a.cost = static_cast<T *>(c.cost);
+  a.tv_stride = c.tv_stride;
+  a.effort = T(c.effort_weight);
   const size_t smem = (size_t)kWarps * OscSmem<T, N, ORTHO, KD>::kElems * sizeof(T);
-  auto kern = rollout_kernel<T, N, ORTHO, KD, PLAIN>;
+  auto kern = rollout_kernel<T, N, ORTHO, KD, PLAIN, RolloutPathArgs<T>>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, O, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO, int KD>
+int rollout_path_go(const ChainHost &h, const abrb_osc_params &p, const RolloutPathCall &c) {
+  // as in generate: a path velocity needs the general instantiation; a shared or per-trajectory path does not matter
+  if (osc_plain(p, N, c.frame, KD, c.tv != nullptr, c.ierr != nullptr))
+    return rollout_path_launch<T, N, ORTHO, KD, true>(h, p, c);
+  return rollout_path_launch<T, N, ORTHO, KD, false>(h, p, c);
+}
+
+template <typename T, int N, bool ORTHO, int KD, bool PLAIN>
+int rollout_launch(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  OscK<T, N> O;
+  fill_osc<T, N>(p, c.frame, c.xoff, O);
+  RolloutArgs<T> a;
+  fill_rollout_args<T>(c, a);
+  const size_t smem = (size_t)kWarps * OscSmem<T, N, ORTHO, KD>::kElems * sizeof(T);
+  auto kern = rollout_kernel<T, N, ORTHO, KD, PLAIN, RolloutArgs<T>>;
   cudaError_t e = set_smem(kern, smem);
   if (e != cudaSuccess) return (int)e;
   kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, O, a);
@@ -812,6 +880,11 @@ int launch_osc<ABRB_N>(const ChainHost &h, const abrb_osc_params &p, const OscCa
 template <>
 int launch_rollout<ABRB_N>(const ChainHost &h, const abrb_osc_params &p, const RolloutCall &c) {
   ABRB_OSC_DISPATCH(rollout_go, h, p, c);
+}
+
+template <>
+int launch_rollout_path<ABRB_N>(const ChainHost &h, const abrb_osc_params &p, const RolloutPathCall &c) {
+  ABRB_OSC_DISPATCH(rollout_path_go, h, p, c);
 }
 
 template <>

@@ -288,6 +288,41 @@ int abrb_osc_rollout_f32(const abrb_osc *c, int frame_id, const double *x_off, f
                          float *q_traj, float *dq_traj, float *u_traj, float *integrated_error, int64_t B,
                          void *stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Path-following rollout (MPC over a reference trajectory): the closed loop of abrb_osc_rollout_*, but step t
+ * drives towards the path's row p_t (x, y, z, Euler a, b, g, as generate's target) with target velocity v_t,
+ * and the control point's track and one tracking cost per trajectory are recorded.  For t = 0 .. steps-1:
+ *     x_t      = position of the control point (frame_id + x_off) at q_t
+ *     u_t      = OSC.generate(q_t, dq_t, target = p_t, target_velocity = v_t)
+ *                (v_t all zero or path_velocity NULL: the -kv M dq law, as generate)
+ *     ddq_t    = M(q_t)^-1 (u_t + g(q_t) - C(q_t, dq_t) dq_t)
+ *     dq_{t+1} = dq_t + ddq_t dt;   q_{t+1} = q_t + dq_{t+1} dt          (semi-implicit Euler, as the rollout)
+ *     cost    += |x_t - p_t[0:3]|^2 + effort_weight |u_t|^2              (in order of t, in the call's precision;
+ *                                                                          position rows even when not controlled)
+ * x_traj[t] and u_traj[t] belong to the state BEFORE step t; q_traj[t] and dq_traj[t] hold the state AFTER it.
+ *   q, dq          (B,n) in/out (final state)
+ *   path           path_stride 6: (steps, B, 6), element (t, b, c) at path[(t*B + b)*6 + c] (one path per trajectory);
+ *                  path_stride 0: (steps, 6), element (t, c) at path[t*6 + c] (one path shared by all)
+ *   path_velocity  NULL or laid out like path per pv_stride (0 or 6)
+ *   q_traj / dq_traj / u_traj: NULL or (steps, B, n);   x_traj: NULL or (steps, B, 3);   cost: NULL or (B,)
+ *   effort_weight  finite, >= 0 (double for both precisions, as dt)
+ *   integrated_error: (B,6) in/out, given if and only if ki != 0; the rollout starts from it and leaves it updated
+ * steps == 0 leaves q, dq unchanged and writes cost = 0; B == 0 does nothing.  Arguments are checked before any
+ * device work: ABRB_EINVAL (NULL controller, q, dq, or path when steps > 0; strides other than 0 or 6; negative
+ * steps or B; effort_weight negative or not finite; integrated_error / ki mismatch; misaligned pointers),
+ * ABRB_EFRAME (bad frame id).
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_osc_rollout_path_f64(const abrb_osc *c, int frame_id, const double *x_off, double *q, double *dq,
+                              const double *path, int path_stride, const double *path_velocity, int pv_stride,
+                              int steps, double dt, double effort_weight,
+                              double *q_traj, double *dq_traj, double *u_traj, double *x_traj, double *cost,
+                              double *integrated_error, int64_t B, void *stream);
+int abrb_osc_rollout_path_f32(const abrb_osc *c, int frame_id, const double *x_off, float *q, float *dq,
+                              const float *path, int path_stride, const float *path_velocity, int pv_stride,
+                              int steps, double dt, double effort_weight,
+                              float *q_traj, float *dq_traj, float *u_traj, float *x_traj, float *cost,
+                              float *integrated_error, int64_t B, void *stream);
+
 /* Kernel launch counter for this process (every launch of a libabrb kernel increments it). */
 int64_t abrb_launch_count(void);
 
