@@ -244,6 +244,120 @@ class BaseConfig:
         """Inverse transform [[R^T, -R^T t], [0, 1]] (base_config.py:394-415; ``x`` is unused there too)."""
         return self._one("T_inv", q, name=name)
 
+    # ------------------------------------------------------------------ the plant (include/abrb.h, abrb_plant_*)
+    def _on_device(self, q, dq):
+        """-> (q, dq as CUDA tensors (B, n), single?, 'torch' or 'numpy', f32?); NumPy is staged through the current
+        device."""
+        from ..controllers import _batch
+
+        qa, dqa, single, kind, f32 = _batch.prep_state(self, q, dq)
+        if kind == "numpy":
+            dev = torch.device("cuda", torch.cuda.current_device())
+            qa, dqa = torch.as_tensor(qa).to(dev), torch.as_tensor(dqa).to(dev)
+        return qa, dqa, single, kind, f32
+
+    def _dynamics(self, q, dq, x, what, fns):
+        qa, dqa, single, kind, f32 = self._on_device(q, dq)
+        B, n = qa.shape
+        xa = (x if _is_torch(x) else torch.as_tensor(np.asarray(x, dtype=np.float64))).to(device=qa.device,
+                                                                                            dtype=qa.dtype)
+        if tuple(xa.shape) != ((n,) if single else (B, n)):
+            raise ValueError(f"{what} must have the shape of q, ({n},) or ({B}, {n}), got {tuple(xa.shape)}")
+        xa = xa.reshape(B, n).contiguous()
+        out = torch.empty_like(qa)
+        fn = getattr(_lib.lib(), fns[1] if f32 else fns[0])
+        with torch.cuda.device(qa.device):
+            _lib.check(fn(self._handle, qa.data_ptr(), dqa.data_ptr(), xa.data_ptr(), out.data_ptr(), B,
+                          torch.cuda.current_stream(qa.device).cuda_stream))
+        if kind == "numpy":
+            out = out.cpu().numpy()
+        return out[0] if single else out
+
+    def forward_dynamics(self, q, dq, u):
+        """Joint accelerations under the torque ``u``: ``ddq = M(q)^-1 (u + g(q) - C(q, dq) dq)``, the plant of the
+        rollouts (``g`` is the gravity force the controllers subtract, so ``u = -g`` holds the arm still).
+        ``q, dq, u`` are ``(n,)`` or ``(B, n)``; CUDA tensors in -> CUDA tensors out, NumPy in -> NumPy out."""
+        return self._dynamics(q, dq, u, "u", ("abrb_forward_dynamics_f64", "abrb_forward_dynamics_f32"))
+
+    def inverse_dynamics(self, q, dq, ddq):
+        """Torque that produces ``ddq``: ``u = M(q) ddq + C(q, dq) dq - g(q)`` (the inverse of ``forward_dynamics``),
+        e.g. the feedforward torque of a planned joint trajectory.  Shapes and types as ``forward_dynamics``."""
+        return self._dynamics(q, dq, ddq, "ddq", ("abrb_inverse_dynamics_f64", "abrb_inverse_dynamics_f32"))
+
+    def simulate(self, q, dq, u, dt=1e-3, path=None, effort_weight=0.0, compensate_gravity=False, ref_frame="EE",
+                 xyz_offset=None, record=("q", "dq", "u", "x")):
+        """Open-loop rollout of the plant under the torque sequence ``u`` on the GPU (abrb_plant_rollout_*).  For each
+        step ``t = 0 .. S-1``, with the semi-implicit Euler step of the reference (arms/twojoint/arm_sim.py:131-132)::
+
+            tau_t = u[t]                    (or u[t] - g(q_t) with compensate_gravity: the residual-torque form)
+            x_t   = Tx(ref_frame, q_t, x=xyz_offset)
+            ddq   = M^-1 (tau_t + g - C dq_t);  dq_{t+1} = dq_t + ddq dt;  q_{t+1} = q_t + dq_{t+1} dt
+            cost += |x_t - path[t, :3]|^2 (with a path) + effort_weight * |tau_t|^2
+
+        ``u`` is ``(S, n)`` (one sequence for every trajectory) or ``(S, B, n)``; ``path`` is None, ``(S, 6)`` or
+        ``(S, B, 6)`` as in ``OSC.rollout_path`` (only columns 0-2 are used).  Returns ``(q_final, dq_final, traj,
+        cost)`` with the records of ``OSC.rollout_path``: ``traj[k]`` for k in ``record`` is ``(S, B, n)`` (``"x"``:
+        ``(S, B, 3)``); ``traj["x"][t]`` and ``traj["u"][t]`` (the applied ``tau_t``) belong to the state before step
+        t, ``traj["q"][t]`` and ``traj["dq"][t]`` to the state after it; ``cost`` is ``(B,)``.  ``record=()`` is the
+        allocation-light form for sampling-based MPC, e.g. MPPI around a nominal torque plan::
+
+            _, _, _, cost = rc.simulate(q0, dq0, u_nominal + noise, path=P, record=())    # noise (S, B, n)
+
+        Fed the ``traj["u"]`` that ``OSC.rollout_path`` recorded, with the same start, path and effort weight, it gives
+        back that rollout's track and cost, so closed-loop and open-loop candidates are scored alike::
+
+            qf, dqf, tr, c = osc.rollout_path(q0, dq0, P, effort_weight=w)
+            qs, dqs, ts, cs = rc.simulate(q0, dq0, tr["u"], path=P, effort_weight=w)       # ts["x"] == tr["x"]
+
+        CUDA tensors in -> CUDA tensors out; NumPy in -> NumPy out.  A single state ``q`` of shape ``(n,)`` takes an
+        ``(S, n)`` sequence and returns ``(S, n)`` records and a scalar cost."""
+        from ..controllers import _batch
+
+        qa, dqa, single, kind, f32 = self._on_device(q, dq)
+        if kind == "torch":
+            qa, dqa = qa.clone(), dqa.clone()
+        B, n = qa.shape
+
+        def rows(x, width, what):
+            t = x if _is_torch(x) else torch.as_tensor(np.asarray(x, dtype=np.float64))
+            t = t.to(device=qa.device, dtype=qa.dtype).contiguous()
+            if t.dim() == 2 and t.shape[1] == width:
+                return t, 0
+            if t.dim() == 3 and t.shape[1:] == (B, width):
+                return t, width
+            raise ValueError(f"{what} must have shape (S, {width}) or (S, {B}, {width})")
+
+        ua, ustride = rows(u, n, "u")
+        steps = ua.shape[0]
+        pth, pstride = (None, 0)
+        if path is not None:
+            pth, pstride = rows(path, 6, "path")
+            if pth.shape[0] != steps:
+                raise ValueError(f"path has {pth.shape[0]} steps, u has {steps}")
+        fid = self.frame_id(ref_frame)
+        xo = None
+        if xyz_offset is not None and not np.allclose(np.asarray(xyz_offset, dtype=float), 0):
+            xo = (C.c_double * 3)(*[float(v) for v in np.asarray(xyz_offset, dtype=float).reshape(3)])
+        for k in record:
+            if k not in ("q", "dq", "u", "x"):
+                raise ValueError(f"simulate can record 'q', 'dq', 'u' and 'x', not {k!r}")
+        traj = {k: torch.empty((steps, B, 3 if k == "x" else n), dtype=qa.dtype, device=qa.device) for k in record}
+        cost = torch.empty((B,), dtype=qa.dtype, device=qa.device)
+        L = _lib.lib()
+        fn = L.abrb_plant_rollout_f32 if f32 else L.abrb_plant_rollout_f64
+        with torch.cuda.device(qa.device):
+            _lib.check(fn(self._handle, fid, xo, qa.data_ptr(), dqa.data_ptr(), ua.data_ptr(), ustride,
+                          1 if compensate_gravity else 0, _batch.ptr(pth), pstride, int(steps), float(dt),
+                          float(effort_weight), _batch.ptr(traj.get("q")), _batch.ptr(traj.get("dq")),
+                          _batch.ptr(traj.get("u")), _batch.ptr(traj.get("x")), cost.data_ptr(), B,
+                          torch.cuda.current_stream(qa.device).cuda_stream))
+        if kind == "numpy":
+            qa, dqa, cost = qa.cpu().numpy(), dqa.cpu().numpy(), cost.cpu().numpy()
+            traj = {k: v.cpu().numpy() for k, v in traj.items()}
+        if single:
+            return qa[0], dqa[0], {k: v[:, 0] for k, v in traj.items()}, cost[0]
+        return qa, dqa, traj, cost
+
 
 def builtin_config(arm, **kwargs):
     """Config for one of the arms shipped with the reference: 'ur5', 'jaco2', 'threejoint', 'twojoint'."""

@@ -111,6 +111,34 @@ struct IkCall {
   cudaStream_t stream;
 };
 
+// abrb_plant_rollout_*: open-loop rollout of the plant under a given torque sequence
+struct PlantCall {
+  int frame;
+  const double *xoff;  // host, 3 values or nullptr
+  void *q, *dq;        // device, in/out
+  const void *u;       // (steps, B, n) for u_stride n, (steps, n) for 0
+  int u_stride;
+  int compensate_gravity;
+  const void *path;    // (steps, B, 6) for path_stride 6, (steps, 6) for 0, or nullptr
+  int path_stride;
+  int steps;
+  double dt, effort_weight;
+  void *q_traj, *dq_traj, *u_traj, *x_traj, *cost;  // each nullptr or device
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+
+// abrb_forward_dynamics_* (kind 0: in = u, out = ddq) and abrb_inverse_dynamics_* (kind 1: in = ddq, out = u)
+struct DynCall {
+  int kind;
+  const void *q, *dq, *in;
+  void *out;
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+
 // Each returns a cudaError_t (0 = success).  Defined once per joint count in kernels.cu (-DABRB_N=<n>).
 template <int N> int launch_rbd(const ChainHost &h, const RbdCall &c);
 template <int N> int launch_osc(const ChainHost &h, const abrb_osc_params &p, const OscCall &c);
@@ -120,6 +148,8 @@ template <int N> int launch_null(const ChainHost &h, const abrb_null_params &z, 
 template <int N> int launch_ctrl(const ChainHost &h, const CtrlCall &c);
 template <int N> int launch_sliding(const ChainHost &h, const SlidingCall &c);
 template <int N> int launch_ik(const ChainHost &h, const IkCall &c);
+template <int N> int launch_plant(const ChainHost &h, const PlantCall &c);
+template <int N> int launch_dyn(const ChainHost &h, const DynCall &c);
 
 void count_launch();
 

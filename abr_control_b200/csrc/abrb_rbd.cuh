@@ -104,4 +104,103 @@ ABRB_HD void rbd_state(const ChainK<T, N> &P, const T *q, const T *dq, int frame
   }
 }
 
+// ------------------------------------------------------------------------------------------------ the plant
+// The rollouts' plant (reference semi-implicit Euler, arms/twojoint/arm_sim.py:131-132) on its own:
+//     ddq = M(q)^-1 (tau + g(q) - C(q, dq) dq),   u = M(q) ddq + C(q, dq) dq - g(q)
+// g is the generalized gravity force the controllers subtract (base_config.py:417-468) and C dq the product
+// dynamics_Mg<T, N, true> returns.  The operations and their order are those of osc_eval's PLANT branch, so a torque
+// sequence recorded by a closed-loop rollout replays to the same track.
+
+// M (full, symmetric), g and C dq of the state whose walk K holds
+template <typename T, int N, class K_>
+ABRB_HD void plant_terms(const ChainK<T, N> &P, const T *dq, T (*M)[N], T *g, T *cdq, K_ &K) {
+  K.sync();
+  dynamics_Mg<T, N, true>(P, K, dq, M, g, cdq);
+  ABRB_UNROLL
+  for (int a = 0; a < N; ++a)
+    ABRB_UNROLL
+  for (int b = 0; b < N; ++b)
+    if (b < a) M[a][b] = M[b][a];
+}
+
+// Forward dynamics of one state: ddq = M^-1 (u + g - C dq)
+template <typename T, int N, class K_>
+ABRB_HD void forward_dynamics_state(const ChainK<T, N> &P, const T *q, const T *dq, const T *u, T *ddq, K_ &K) {
+  K.sync();
+  walk<T, N>(P, q, 0, K);
+  T M[N][N], Mi[N], g[N], cdq[N];
+  plant_terms<T, N>(P, dq, M, g, cdq, K);
+  K.sync();
+  chol<T, N>(M, Mi);
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) ddq[k] = u[k] + g[k] - cdq[k];
+  fwd_solve<T, N>(M, Mi, ddq);
+  bwd_solve<T, N>(M, Mi, ddq);
+}
+
+// Inverse dynamics of one state: u = M ddq + C dq - g
+template <typename T, int N, class K_>
+ABRB_HD void inverse_dynamics_state(const ChainK<T, N> &P, const T *q, const T *dq, const T *ddq, T *u, K_ &K) {
+  K.sync();
+  walk<T, N>(P, q, 0, K);
+  T M[N][N], g[N], cdq[N];
+  plant_terms<T, N>(P, dq, M, g, cdq, K);
+  ABRB_UNROLL
+  for (int a = 0; a < N; ++a) {
+    T s = T(0);
+    ABRB_UNROLL
+    for (int b = 0; b < N; ++b) s += M[a][b] * ddq[b];
+    u[a] = s + cdq[a] - g[a];
+  }
+}
+
+// Row t of trajectory b of a torque sequence of abrb_plant_rollout_*: (steps, B, N) when stride != 0 (== N), one
+// (steps, N) sequence for every trajectory when stride == 0.
+template <typename T, int N>
+ABRB_HD const T *torque_row(const T *u, int stride, int t, int64_t B, int64_t b) {
+  return u + (stride != 0 ? ((int64_t)t * B + b) * N : (int64_t)t * N);
+}
+
+// One step of the open-loop plant rollout (plant_kernel), for the torque row `u` and the path row `p` (3 values used,
+// or nullptr):
+//     tau = u, or u - g with comp_g (the residual-torque form);  x = control point (frame + xoff) at q
+//     ddq = M^-1 (tau + g - C dq);  dq += ddq dt;  q += dq dt
+//     cost += |x - p[:3]|^2 (with a path) + effort |tau|^2
+// `tau` and `x` belong to the state BEFORE the update, as in rollout_step.
+template <typename T, int N, class K_>
+ABRB_HD void plant_step(const ChainK<T, N> &P, int frame, const T *xoff, T *q, T *dq, const T *u, bool comp_g,
+                        const T *p, T dt, T effort, T *tau, T *x, T &cost, K_ &K) {
+  K.sync();
+  walk<T, N>(P, q, frame, K);
+  K.sync();
+  frame_point(K.F, xoff, x);
+  T M[N][N], Mi[N], g[N], cdq[N], rhs[N];
+  plant_terms<T, N>(P, dq, M, g, cdq, K);
+  K.sync();
+  chol<T, N>(M, Mi);
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) {
+    tau[k] = comp_g ? u[k] - g[k] : u[k];
+    rhs[k] = tau[k] + g[k] - cdq[k];
+  }
+  fwd_solve<T, N>(M, Mi, rhs);
+  bwd_solve<T, N>(M, Mi, rhs);
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) {
+    dq[k] += rhs[k] * dt;
+    q[k] += dq[k] * dt;
+  }
+  T ex = T(0), eu = T(0);
+  if (p != nullptr) {
+    ABRB_UNROLL
+    for (int c = 0; c < 3; ++c) {
+      const T d = x[c] - p[c];
+      ex += d * d;
+    }
+  }
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) eu += tau[k] * tau[k];
+  cost += ex + effort * eu;
+}
+
 }  // namespace abrb

@@ -1055,4 +1055,103 @@ int abrb_osc_rollout_path_f32(const abrb_osc *c, int frame_id, const double *x_o
                           effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, integrated_error, B, stream, true);
 }
 
+// ------------------------------------------------------------------------------------------------ plant
+static int plant_dynamics(const abrb_model *m, const void *q, const void *dq, const void *in, void *out, int64_t B,
+                          void *stream, bool f32, int kind) {
+  const char *who = kind == 0 ? "abrb_forward_dynamics" : "abrb_inverse_dynamics";
+  const char *in_name = kind == 0 ? "u" : "ddq", *out_name = kind == 0 ? "ddq" : "u";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (B == 0) return ABRB_OK;
+  const void *ptrs[] = {q, dq, in, out};
+  const char *names[] = {"q", "dq", in_name, out_name};
+  for (int i = 0; i < 4; ++i) {
+    if (!ptrs[i]) return fail(ABRB_EINVAL, w + ": NULL " + names[i]);
+    if (!aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  }
+  int rc = ensure_device();
+  if (rc) return rc;
+  DynCall k{kind, q, dq, in, out, B, f32, (cudaStream_t)stream};
+  int e = cudaErrorInvalidValue;
+  switch (m->host.n) {
+#define X(j) case j: e = launch_dyn<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_forward_dynamics_f64(const abrb_model *m, const double *q, const double *dq, const double *u, double *ddq,
+                              int64_t B, void *stream) {
+  return plant_dynamics(m, q, dq, u, ddq, B, stream, false, 0);
+}
+int abrb_forward_dynamics_f32(const abrb_model *m, const float *q, const float *dq, const float *u, float *ddq,
+                              int64_t B, void *stream) {
+  return plant_dynamics(m, q, dq, u, ddq, B, stream, true, 0);
+}
+int abrb_inverse_dynamics_f64(const abrb_model *m, const double *q, const double *dq, const double *ddq, double *u,
+                              int64_t B, void *stream) {
+  return plant_dynamics(m, q, dq, ddq, u, B, stream, false, 1);
+}
+int abrb_inverse_dynamics_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq, float *u,
+                              int64_t B, void *stream) {
+  return plant_dynamics(m, q, dq, ddq, u, B, stream, true, 1);
+}
+
+static int plant_rollout(const abrb_model *m, int frame_id, const double *x_off, void *q, void *dq, const void *u,
+                         int u_stride, int compensate_gravity, const void *path, int path_stride, int steps, double dt,
+                         double effort_weight, void *q_traj, void *dq_traj, void *u_traj, void *x_traj, void *cost,
+                         int64_t B, void *stream, bool f32) {
+  const char *who = "abrb_plant_rollout";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (steps < 0) return fail(ABRB_EINVAL, w + ": steps < 0");
+  const int n = m->host.n;
+  if (frame_id < 0 || frame_id > 2 * n + 1) return fail(ABRB_EFRAME, w + ": invalid frame id");
+  if (u_stride != 0 && u_stride != n) return fail(ABRB_EINVAL, w + ": u_stride must be 0 or n_joints");
+  if (path_stride != 0 && path_stride != 6) return fail(ABRB_EINVAL, w + ": path_stride must be 0 or 6");
+  if (!std::isfinite(effort_weight) || effort_weight < 0.0)
+    return fail(ABRB_EINVAL, w + ": effort_weight must be finite and >= 0");
+  if (B == 0) return ABRB_OK;
+  if (!q) return fail(ABRB_EINVAL, w + ": NULL q");
+  if (!dq) return fail(ABRB_EINVAL, w + ": NULL dq");
+  if (steps > 0 && !u) return fail(ABRB_EINVAL, w + ": NULL u");
+  const void *ptrs[] = {q, dq, u, path, q_traj, dq_traj, u_traj, x_traj, cost};
+  const char *names[] = {"q", "dq", "u", "path", "q_traj", "dq_traj", "u_traj", "x_traj", "cost"};
+  for (int i = 0; i < 9; ++i)
+    if (ptrs[i] && !aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  if (steps == 0) {  // nothing to step: q and dq stay as they are, the cost is zero
+    int e = cost ? (int)cudaMemsetAsync(cost, 0, (size_t)B * (f32 ? 4 : 8), (cudaStream_t)stream) : 0;
+    return e ? cuda_fail(e, who) : ABRB_OK;
+  }
+  PlantCall k{frame_id, x_off, q, dq, u, u_stride, compensate_gravity, path, path_stride, steps, dt, effort_weight,
+              q_traj, dq_traj, u_traj, x_traj, cost, B, f32, (cudaStream_t)stream};
+  int e = cudaErrorInvalidValue;
+  switch (n) {
+#define X(j) case j: e = launch_plant<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_plant_rollout_f64(const abrb_model *m, int frame_id, const double *x_off, double *q, double *dq,
+                           const double *u, int u_stride, int compensate_gravity, const double *path, int path_stride,
+                           int steps, double dt, double effort_weight, double *q_traj, double *dq_traj, double *u_traj,
+                           double *x_traj, double *cost, int64_t B, void *stream) {
+  return plant_rollout(m, frame_id, x_off, q, dq, u, u_stride, compensate_gravity, path, path_stride, steps, dt,
+                       effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream, false);
+}
+int abrb_plant_rollout_f32(const abrb_model *m, int frame_id, const double *x_off, float *q, float *dq, const float *u,
+                           int u_stride, int compensate_gravity, const float *path, int path_stride, int steps,
+                           double dt, double effort_weight, float *q_traj, float *dq_traj, float *u_traj,
+                           float *x_traj, float *cost, int64_t B, void *stream) {
+  return plant_rollout(m, frame_id, x_off, q, dq, u, u_stride, compensate_gravity, path, path_stride, steps, dt,
+                       effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream, true);
+}
+
 }  // extern "C"

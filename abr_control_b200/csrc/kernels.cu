@@ -593,6 +593,106 @@ ik_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ IkArgs
   }
 }
 
+template <typename T>
+struct PlantArgs {
+  T *q, *dq;
+  const T *u;     // torques, row t of trajectory b at torque_row(u, u_stride, t, B, b)
+  const T *path;  // (steps, B, 6) (path_stride 6), (steps, 6) (0), or nullptr
+  T *q_traj, *dq_traj, *u_traj, *x_traj, *cost;
+  int64_t B;
+  int u_stride, path_stride, steps, frame, comp_g;
+  T dt, effort;
+  T xoff[3];
+};
+
+// Open-loop plant rollout (abrb_plant_rollout_*): one trajectory per thread, q and dq in registers across the steps,
+// the torque of step t read from the caller's sequence (plant_step, abrb_rbd.cuh).  M is factorised by Cholesky, so
+// there is no cooperative part; the kinematic scratch is the one the rollout kernel uses.
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(kBlock)
+plant_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ PlantArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef WarpSmem<T, N, ORTHO, (N > 3 ? N : 3)> WS;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
+  T *stage = region + WS::kKin;
+  typename KS::type K;
+  KS::bind(K, region, lane);
+  for (int64_t base = (int64_t)blockIdx.x * kBlock; base < a.B; base += (int64_t)gridDim.x * kBlock) {
+    const int64_t warp_b0 = base + warp * 32;
+    if (warp_b0 >= a.B) break;
+    const int64_t rem = a.B - warp_b0;
+    const int nvalid = rem < 32 ? (int)rem : 32;
+    const int64_t b = warp_b0 + (lane < nvalid ? lane : nvalid - 1);
+    T q[N], dq[N], ur[N], tau[N], x[3];
+    T cost = T(0);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      q[k] = a.q[b * N + k];
+      dq[k] = a.dq[b * N + k];
+    }
+    for (int t = 0; t < a.steps; ++t) {
+      // a shared sequence (or path) is one address for the whole warp (a broadcast load), a per-trajectory one a row
+      // per lane
+      const T *ut = torque_row<T, N>(a.u, a.u_stride, t, a.B, b);
+#pragma unroll
+      for (int k = 0; k < N; ++k) ur[k] = ut[k];
+      const T *pt = a.path != nullptr ? path_row(a.path, a.path_stride, t, a.B, b) : nullptr;
+      plant_step<T, N>(P, a.frame, a.xoff, q, dq, ur, a.comp_g != 0, pt, a.dt, a.effort, tau, x, cost, K);
+      const int64_t row0 = (int64_t)t * a.B + warp_b0;
+      if (a.u_traj) store_records<T, N>(a.u_traj, row0, nvalid, tau, stage, lane);
+      if (a.q_traj) store_records<T, N>(a.q_traj, row0, nvalid, q, stage, lane);
+      if (a.dq_traj) store_records<T, N>(a.dq_traj, row0, nvalid, dq, stage, lane);
+      if (a.x_traj) store_records<T, 3>(a.x_traj, row0, nvalid, x, stage, lane);
+    }
+    store_records<T, N>(a.q, warp_b0, nvalid, q, stage, lane);
+    store_records<T, N>(a.dq, warp_b0, nvalid, dq, stage, lane);
+    if (a.cost != nullptr && lane < nvalid) a.cost[b] = cost;
+  }
+}
+
+template <typename T>
+struct DynArgs {
+  const T *q, *dq, *in;  // in: u (kind 0) or ddq (kind 1)
+  T *out;                // ddq (kind 0) or u (kind 1)
+  int64_t B;
+  int kind;
+};
+
+// abrb_forward_dynamics_* (kind 0) and abrb_inverse_dynamics_* (kind 1): one state per thread, grid-stride
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(kBlock)
+dyn_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ DynArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef WarpSmem<T, N, ORTHO, N> WS;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
+  T *stage = region + WS::kKin;
+  typename KS::type K;
+  KS::bind(K, region, lane);
+  for (int64_t base = (int64_t)blockIdx.x * kBlock; base < a.B; base += (int64_t)gridDim.x * kBlock) {
+    const int64_t warp_b0 = base + warp * 32;
+    if (warp_b0 >= a.B) break;
+    const int64_t rem = a.B - warp_b0;
+    const int nvalid = rem < 32 ? (int)rem : 32;
+    const int64_t b = warp_b0 + (lane < nvalid ? lane : nvalid - 1);
+    T q[N], dq[N], in[N], out[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      q[k] = a.q[b * N + k];
+      dq[k] = a.dq[b * N + k];
+      in[k] = a.in[b * N + k];
+    }
+    if (a.kind == 0)
+      forward_dynamics_state<T, N>(P, q, dq, in, out, K);
+    else
+      inverse_dynamics_state<T, N>(P, q, dq, in, out, K);
+    store_records<T, N>(a.out, warp_b0, nvalid, out, stage, lane);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ launch
 // kernel<<<grid, block, smem, stream>>>(args...) with programmatic stream serialization allowed: the launch may be
 // brought onto the SMs while the stream's previous kernel drains; the kernels launched through it (osc_kernel,
@@ -940,6 +1040,70 @@ int ik_go(const ChainHost &h, const IkCall &c) {
   ik_kernel<T, N, ORTHO><<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, a);
   count_launch();
   return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO>
+int plant_go(const ChainHost &h, const PlantCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  PlantArgs<T> a;
+  a.q = static_cast<T *>(c.q);
+  a.dq = static_cast<T *>(c.dq);
+  a.u = static_cast<const T *>(c.u);
+  a.path = static_cast<const T *>(c.path);
+  a.q_traj = static_cast<T *>(c.q_traj);
+  a.dq_traj = static_cast<T *>(c.dq_traj);
+  a.u_traj = static_cast<T *>(c.u_traj);
+  a.x_traj = static_cast<T *>(c.x_traj);
+  a.cost = static_cast<T *>(c.cost);
+  a.B = c.B;
+  a.u_stride = c.u_stride;
+  a.path_stride = c.path_stride;
+  a.steps = c.steps;
+  a.frame = c.frame;
+  a.comp_g = c.compensate_gravity;
+  a.dt = T(c.dt);
+  a.effort = T(c.effort_weight);
+  for (int i = 0; i < 3; ++i) a.xoff[i] = c.xoff ? T(c.xoff[i]) : T(0);
+  const size_t smem = (size_t)kWarps * WarpSmem<T, N, ORTHO, (N > 3 ? N : 3)>::kElems * sizeof(T);
+  auto kern = plant_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO>
+int dyn_go(const ChainHost &h, const DynCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  DynArgs<T> a;
+  a.q = static_cast<const T *>(c.q);
+  a.dq = static_cast<const T *>(c.dq);
+  a.in = static_cast<const T *>(c.in);
+  a.out = static_cast<T *>(c.out);
+  a.B = c.B;
+  a.kind = c.kind;
+  const size_t smem = (size_t)kWarps * WarpSmem<T, N, ORTHO, N>::kElems * sizeof(T);
+  auto kern = dyn_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <>
+int launch_plant<ABRB_N>(const ChainHost &h, const PlantCall &c) {
+  if (c.f32) return h.ortho ? plant_go<float, ABRB_N, true>(h, c) : plant_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? plant_go<double, ABRB_N, true>(h, c) : plant_go<double, ABRB_N, false>(h, c);
+}
+
+template <>
+int launch_dyn<ABRB_N>(const ChainHost &h, const DynCall &c) {
+  if (c.f32) return h.ortho ? dyn_go<float, ABRB_N, true>(h, c) : dyn_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? dyn_go<double, ABRB_N, true>(h, c) : dyn_go<double, ABRB_N, false>(h, c);
 }
 
 template <>

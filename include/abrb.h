@@ -323,6 +323,58 @@ int abrb_osc_rollout_path_f32(const abrb_osc *c, int frame_id, const double *x_o
                               float *q_traj, float *dq_traj, float *u_traj, float *x_traj, float *cost,
                               float *integrated_error, int64_t B, void *stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * The rollouts' plant on its own, for torques from anywhere (sampling-based MPC in torque space, other
+ * controllers, replay of a recorded u_traj, feedforward torques of a planned joint trajectory).  It is the plant
+ * of abrb_osc_rollout_* (semi-implicit Euler as arms/twojoint/arm_sim.py:131-132), with g the generalized gravity
+ * force the controllers subtract (base_config.py:417-468) and C dq the rollout's Coriolis product:
+ *     forward dynamics   ddq = M(q)^-1 (u + g(q) - C(q, dq) dq)
+ *     inverse dynamics   u   = M(q) ddq + C(q, dq) dq - g(q)
+ *   q, dq, u, ddq (B,n).  B == 0 does nothing.  ABRB_EINVAL: NULL model or array, B < 0, misaligned pointers.
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_forward_dynamics_f64(const abrb_model *m, const double *q, const double *dq, const double *u,
+                              double *ddq, int64_t B, void *stream);
+int abrb_forward_dynamics_f32(const abrb_model *m, const float *q, const float *dq, const float *u,
+                              float *ddq, int64_t B, void *stream);
+int abrb_inverse_dynamics_f64(const abrb_model *m, const double *q, const double *dq, const double *ddq,
+                              double *u, int64_t B, void *stream);
+int abrb_inverse_dynamics_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq,
+                              float *u, int64_t B, void *stream);
+
+/* Open-loop plant rollout under a given torque sequence u_t.  For t = 0 .. steps-1:
+ *     tau_t    = u_t                       (compensate_gravity == 0)
+ *     tau_t    = u_t - g(q_t)              (compensate_gravity != 0: u_t is the residual torque MPPI samples around)
+ *     x_t      = position of the control point (frame_id + x_off) at q_t
+ *     ddq_t    = M(q_t)^-1 (tau_t + g(q_t) - C(q_t, dq_t) dq_t)
+ *     dq_{t+1} = dq_t + ddq_t dt;   q_{t+1} = q_t + dq_{t+1} dt
+ *     cost    += |x_t - p_t[0:3]|^2 (with a path only) + effort_weight |tau_t|^2   (in order of t, in the call's
+ *                                                                                  precision)
+ * The records follow abrb_osc_rollout_path_*: x_traj[t] and u_traj[t] (the applied tau_t) belong to the state
+ * BEFORE step t, q_traj[t] and dq_traj[t] hold the state AFTER it; the cost is the same sum.  So the u_traj of a
+ * closed-loop path rollout, fed back here with the same path and effort_weight, gives back that rollout's track and
+ * cost, and closed-loop and open-loop candidates are scored alike.
+ *   q, dq          (B,n) in/out (final state)
+ *   u              u_stride n: (steps, B, n), element (t, b, k) at u[(t*B + b)*n + k] (one sequence per trajectory);
+ *                  u_stride 0: (steps, n), element (t, k) at u[t*n + k] (one sequence shared by all)
+ *   path           NULL or laid out as in abrb_osc_rollout_path_* per path_stride (6 or 0); columns 0-2 are used
+ *   q_traj / dq_traj / u_traj: NULL or (steps, B, n);   x_traj: NULL or (steps, B, 3);   cost: NULL or (B,)
+ *   effort_weight  finite, >= 0 (double for both precisions, as dt)
+ * steps == 0 leaves q, dq unchanged and writes cost = 0; B == 0 does nothing.  Arguments are checked before any
+ * device work: ABRB_EINVAL (NULL model, q, dq, or u when steps > 0; u_stride other than 0 or n; path_stride other
+ * than 0 or 6; negative steps or B; effort_weight negative or not finite; misaligned pointers), ABRB_EFRAME (bad
+ * frame id).
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_plant_rollout_f64(const abrb_model *m, int frame_id, const double *x_off, double *q, double *dq,
+                           const double *u, int u_stride, int compensate_gravity,
+                           const double *path, int path_stride, int steps, double dt, double effort_weight,
+                           double *q_traj, double *dq_traj, double *u_traj, double *x_traj, double *cost,
+                           int64_t B, void *stream);
+int abrb_plant_rollout_f32(const abrb_model *m, int frame_id, const double *x_off, float *q, float *dq,
+                           const float *u, int u_stride, int compensate_gravity,
+                           const float *path, int path_stride, int steps, double dt, double effort_weight,
+                           float *q_traj, float *dq_traj, float *u_traj, float *x_traj, float *cost,
+                           int64_t B, void *stream);
+
 /* Kernel launch counter for this process (every launch of a libabrb kernel increments it). */
 int64_t abrb_launch_count(void);
 
