@@ -35,6 +35,11 @@ _dyn = [_VP, _VP, _VP, _VP, _VP, _I64, _VP]  # m, q, dq, u | ddq, ddq | u, B, st
 # m, frame_id, x_off, q, dq, u, u_stride, compensate_gravity, path, path_stride, steps, dt, effort_weight,
 # q_traj, dq_traj, u_traj, x_traj, cost, B, stream
 _plant = [_VP, _I, _VP, _VP, _VP, _VP, _I, _I, _VP, _I, _I, _D, _D, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
+# m, q, dq, u | ddq, d_q, d_dq, d_u | d_ddq, B, stream
+_djac = [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
+# m, frame_id, x_off, q0, dq0, u, u_stride, compensate_gravity, path, path_stride, steps, dt, effort_weight,
+# q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj, gu, gq0, gdq0, B, stream
+_vjp = [_VP, _I, _VP, _VP, _VP, _VP, _I, _I, _VP, _I, _I, _D, _D] + [_VP] * 12 + [_I64, _VP]
 SIGNATURES = {
     "abrb_version": (_I, []),
     "abrb_last_error": (_CP, []),
@@ -87,6 +92,12 @@ SIGNATURES = {
     "abrb_inverse_dynamics_f32": (_I, _dyn),
     "abrb_plant_rollout_f64": (_I, _plant),
     "abrb_plant_rollout_f32": (_I, _plant),
+    "abrb_forward_dynamics_derivatives_f64": (_I, _djac),
+    "abrb_forward_dynamics_derivatives_f32": (_I, _djac),
+    "abrb_inverse_dynamics_derivatives_f64": (_I, _djac),
+    "abrb_inverse_dynamics_derivatives_f32": (_I, _djac),
+    "abrb_plant_rollout_vjp_f64": (_I, _vjp),
+    "abrb_plant_rollout_vjp_f32": (_I, _vjp),
     "abrb_launch_count": (_I64, []),
 }
 

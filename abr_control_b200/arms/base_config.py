@@ -36,6 +36,11 @@ def _is_torch(x):
     return torch is not None and isinstance(x, torch.Tensor)
 
 
+def _is_torch_grad(*xs):
+    """grad mode is on and one of ``xs`` is a tensor that requires grad (the differentiable path of the plant)"""
+    return torch.is_grad_enabled() and any(_is_torch(x) and x.requires_grad for x in xs)
+
+
 class BaseConfig:
     """Batched arm model built from a flat chain descriptor (see ``abr_control_b200/arms/data/*.json``).
 
@@ -273,16 +278,58 @@ class BaseConfig:
             out = out.cpu().numpy()
         return out[0] if single else out
 
+    def _derivatives(self, q, dq, x, kind, want_in=True):
+        what = "u" if kind == 0 else "ddq"
+        qa, dqa, single, hkind, f32 = self._on_device(q, dq)
+        B, n = qa.shape
+        xa = (x if _is_torch(x) else torch.as_tensor(np.asarray(x, dtype=np.float64))).to(device=qa.device,
+                                                                                            dtype=qa.dtype)
+        if tuple(xa.shape) != ((n,) if single else (B, n)):
+            raise ValueError(f"{what} must have the shape of q, ({n},) or ({B}, {n}), got {tuple(xa.shape)}")
+        xa = xa.reshape(B, n).contiguous()
+        d = [torch.empty((B, n, n), dtype=qa.dtype, device=qa.device) for _ in range(3 if want_in else 2)]
+        name = "abrb_forward_dynamics_derivatives" if kind == 0 else "abrb_inverse_dynamics_derivatives"
+        fn = getattr(_lib.lib(), name + ("_f32" if f32 else "_f64"))
+        with torch.cuda.device(qa.device):
+            _lib.check(fn(self._handle, qa.data_ptr(), dqa.data_ptr(), xa.data_ptr(), d[0].data_ptr(), d[1].data_ptr(),
+                          d[2].data_ptr() if want_in else None, B, torch.cuda.current_stream(qa.device).cuda_stream))
+        if hkind == "numpy":
+            d = [t.cpu().numpy() for t in d]
+        if single:
+            d = [t[0] for t in d]
+        return tuple(d) if want_in else (d[0], d[1], None)
+
     def forward_dynamics(self, q, dq, u):
         """Joint accelerations under the torque ``u``: ``ddq = M(q)^-1 (u + g(q) - C(q, dq) dq)``, the plant of the
         rollouts (``g`` is the gravity force the controllers subtract, so ``u = -g`` holds the arm still).
-        ``q, dq, u`` are ``(n,)`` or ``(B, n)``; CUDA tensors in -> CUDA tensors out, NumPy in -> NumPy out."""
+        ``q, dq, u`` are ``(n,)`` or ``(B, n)``; CUDA tensors in -> CUDA tensors out, NumPy in -> NumPy out.
+        Differentiable (``torch.autograd``, first order) when grad mode is on and a CUDA tensor input requires grad."""
+        if torch is not None and _is_torch_grad(q, dq, u):
+            from . import _autograd
+
+            return _autograd.dynamics(self, 0, q, dq, u)
         return self._dynamics(q, dq, u, "u", ("abrb_forward_dynamics_f64", "abrb_forward_dynamics_f32"))
 
     def inverse_dynamics(self, q, dq, ddq):
         """Torque that produces ``ddq``: ``u = M(q) ddq + C(q, dq) dq - g(q)`` (the inverse of ``forward_dynamics``),
-        e.g. the feedforward torque of a planned joint trajectory.  Shapes and types as ``forward_dynamics``."""
+        e.g. the feedforward torque of a planned joint trajectory.  Shapes and types as ``forward_dynamics``; likewise
+        differentiable."""
+        if torch is not None and _is_torch_grad(q, dq, ddq):
+            from . import _autograd
+
+            return _autograd.dynamics(self, 1, q, dq, ddq)
         return self._dynamics(q, dq, ddq, "ddq", ("abrb_inverse_dynamics_f64", "abrb_inverse_dynamics_f32"))
+
+    def forward_dynamics_derivatives(self, q, dq, u):
+        """Derivatives of ``forward_dynamics``: ``(d_q, d_dq, d_u)``, each ``(B, n, n)`` (``(n, n)`` for one state) with
+        element ``[b, i, j] = d ddq_i / d x_j``; ``d_u`` is ``M^-1``.  Exact (forward-mode dual numbers through the
+        same device code), not finite differences.  Input and output types as ``forward_dynamics``."""
+        return self._derivatives(q, dq, u, 0)
+
+    def inverse_dynamics_derivatives(self, q, dq, ddq):
+        """Derivatives of ``inverse_dynamics``: ``(d_q, d_dq, d_ddq)``, element ``[b, i, j] = d u_i / d x_j``;
+        ``d_ddq`` is ``M``.  Types and shapes as ``forward_dynamics_derivatives``."""
+        return self._derivatives(q, dq, ddq, 1)
 
     def simulate(self, q, dq, u, dt=1e-3, path=None, effort_weight=0.0, compensate_gravity=False, ref_frame="EE",
                  xyz_offset=None, record=("q", "dq", "u", "x")):
@@ -310,9 +357,22 @@ class BaseConfig:
             qs, dqs, ts, cs = rc.simulate(q0, dq0, tr["u"], path=P, effort_weight=w)       # ts["x"] == tr["x"]
 
         CUDA tensors in -> CUDA tensors out; NumPy in -> NumPy out.  A single state ``q`` of shape ``(n,)`` takes an
-        ``(S, n)`` sequence and returns ``(S, n)`` records and a scalar cost."""
+        ``(S, n)`` sequence and returns ``(S, n)`` records and a scalar cost.
+
+        Differentiable (``torch.autograd``, first order) when grad mode is on and ``q``, ``dq`` or ``u`` is a CUDA
+        tensor that requires grad: gradients reach ``u`` (summed over trajectories for a shared ``(S, n)`` sequence),
+        ``q`` and ``dq`` from the cost, the final state and every returned record, through the adjoint recursion of
+        ``abrb_plant_rollout_vjp_*``.  The path, ``dt`` and ``effort_weight`` are constants; a path that requires
+        grad raises ``NotImplementedError``."""
         from ..controllers import _batch
 
+        if torch is not None and _is_torch(path) and path.requires_grad and torch.is_grad_enabled():
+            raise NotImplementedError("simulate is not differentiable with respect to the path")
+        if torch is not None and _is_torch_grad(q, dq, u):
+            from . import _autograd
+
+            return _autograd.simulate(self, q, dq, u, dt, path, effort_weight, compensate_gravity, ref_frame,
+                                      xyz_offset, record)
         qa, dqa, single, kind, f32 = self._on_device(q, dq)
         if kind == "torch":
             qa, dqa = qa.clone(), dqa.clone()

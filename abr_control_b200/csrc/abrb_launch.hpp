@@ -139,6 +139,37 @@ struct DynCall {
   cudaStream_t stream;
 };
 
+// abrb_forward_dynamics_derivatives_* (kind 0: in = u) and abrb_inverse_dynamics_derivatives_* (kind 1: in = ddq):
+// (B, n, n) derivatives of the output with respect to q, dq and in (d_in may be nullptr)
+struct DynJacCall {
+  int kind;
+  const void *q, *dq, *in;
+  void *d_q, *d_dq, *d_in;
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+
+// abrb_plant_rollout_vjp_*: the rollout's arguments, its recorded states and the cotangents of its outputs (each
+// nullptr or device) -> the cotangents of u (per trajectory), q0 and dq0
+struct PlantVjpCall {
+  int frame;
+  const double *xoff;  // host, 3 values or nullptr
+  const void *q0, *dq0, *u;
+  int u_stride;
+  int compensate_gravity;
+  const void *path;
+  int path_stride;
+  int steps;
+  double dt, effort_weight;
+  const void *q_traj, *dq_traj;
+  const void *g_cost, *g_q, *g_dq, *g_q_traj, *g_dq_traj, *g_u_traj, *g_x_traj;
+  void *gu, *gq0, *gdq0;
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+
 // Each returns a cudaError_t (0 = success).  Defined once per joint count in kernels.cu (-DABRB_N=<n>).
 template <int N> int launch_rbd(const ChainHost &h, const RbdCall &c);
 template <int N> int launch_osc(const ChainHost &h, const abrb_osc_params &p, const OscCall &c);
@@ -150,6 +181,8 @@ template <int N> int launch_sliding(const ChainHost &h, const SlidingCall &c);
 template <int N> int launch_ik(const ChainHost &h, const IkCall &c);
 template <int N> int launch_plant(const ChainHost &h, const PlantCall &c);
 template <int N> int launch_dyn(const ChainHost &h, const DynCall &c);
+template <int N> int launch_dyn_jac(const ChainHost &h, const DynJacCall &c);
+template <int N> int launch_plant_vjp(const ChainHost &h, const PlantVjpCall &c);
 
 void count_launch();
 

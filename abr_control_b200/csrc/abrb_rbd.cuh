@@ -123,14 +123,10 @@ ABRB_HD void plant_terms(const ChainK<T, N> &P, const T *dq, T (*M)[N], T *g, T 
     if (b < a) M[a][b] = M[b][a];
 }
 
-// Forward dynamics of one state: ddq = M^-1 (u + g - C dq)
-template <typename T, int N, class K_>
-ABRB_HD void forward_dynamics_state(const ChainK<T, N> &P, const T *q, const T *dq, const T *u, T *ddq, K_ &K) {
-  K.sync();
-  walk<T, N>(P, q, 0, K);
-  T M[N][N], Mi[N], g[N], cdq[N];
-  plant_terms<T, N>(P, dq, M, g, cdq, K);
-  K.sync();
+// ddq = M^-1 (u + g - C dq) by Cholesky (M is overwritten by its factor): the tail of forward_dynamics_state
+template <typename T, int N>
+ABRB_HD void forward_solve(T (*M)[N], const T *g, const T *cdq, const T *u, T *ddq) {
+  T Mi[N];
   chol<T, N>(M, Mi);
   ABRB_UNROLL
   for (int k = 0; k < N; ++k) ddq[k] = u[k] + g[k] - cdq[k];
@@ -138,13 +134,20 @@ ABRB_HD void forward_dynamics_state(const ChainK<T, N> &P, const T *q, const T *
   bwd_solve<T, N>(M, Mi, ddq);
 }
 
-// Inverse dynamics of one state: u = M ddq + C dq - g
+// Forward dynamics of one state: ddq = M^-1 (u + g - C dq)
 template <typename T, int N, class K_>
-ABRB_HD void inverse_dynamics_state(const ChainK<T, N> &P, const T *q, const T *dq, const T *ddq, T *u, K_ &K) {
+ABRB_HD void forward_dynamics_state(const ChainK<T, N> &P, const T *q, const T *dq, const T *u, T *ddq, K_ &K) {
   K.sync();
   walk<T, N>(P, q, 0, K);
   T M[N][N], g[N], cdq[N];
   plant_terms<T, N>(P, dq, M, g, cdq, K);
+  K.sync();
+  forward_solve<T, N>(M, g, cdq, u, ddq);
+}
+
+// u = M ddq + C dq - g: the tail of inverse_dynamics_state
+template <typename T, int N>
+ABRB_HD void inverse_apply(const T (*M)[N], const T *g, const T *cdq, const T *ddq, T *u) {
   ABRB_UNROLL
   for (int a = 0; a < N; ++a) {
     T s = T(0);
@@ -154,6 +157,16 @@ ABRB_HD void inverse_dynamics_state(const ChainK<T, N> &P, const T *q, const T *
   }
 }
 
+// Inverse dynamics of one state: u = M ddq + C dq - g
+template <typename T, int N, class K_>
+ABRB_HD void inverse_dynamics_state(const ChainK<T, N> &P, const T *q, const T *dq, const T *ddq, T *u, K_ &K) {
+  K.sync();
+  walk<T, N>(P, q, 0, K);
+  T M[N][N], g[N], cdq[N];
+  plant_terms<T, N>(P, dq, M, g, cdq, K);
+  inverse_apply<T, N>(M, g, cdq, ddq, u);
+}
+
 // Row t of trajectory b of a torque sequence of abrb_plant_rollout_*: (steps, B, N) when stride != 0 (== N), one
 // (steps, N) sequence for every trajectory when stride == 0.
 template <typename T, int N>
@@ -161,22 +174,12 @@ ABRB_HD const T *torque_row(const T *u, int stride, int t, int64_t B, int64_t b)
   return u + (stride != 0 ? ((int64_t)t * B + b) * N : (int64_t)t * N);
 }
 
-// One step of the open-loop plant rollout (plant_kernel), for the torque row `u` and the path row `p` (3 values used,
-// or nullptr):
-//     tau = u, or u - g with comp_g (the residual-torque form);  x = control point (frame + xoff) at q
-//     ddq = M^-1 (tau + g - C dq);  dq += ddq dt;  q += dq dt
-//     cost += |x - p[:3]|^2 (with a path) + effort |tau|^2
-// `tau` and `x` belong to the state BEFORE the update, as in rollout_step.
-template <typename T, int N, class K_>
-ABRB_HD void plant_step(const ChainK<T, N> &P, int frame, const T *xoff, T *q, T *dq, const T *u, bool comp_g,
-                        const T *p, T dt, T effort, T *tau, T *x, T &cost, K_ &K) {
-  K.sync();
-  walk<T, N>(P, q, frame, K);
-  K.sync();
-  frame_point(K.F, xoff, x);
-  T M[N][N], Mi[N], g[N], cdq[N], rhs[N];
-  plant_terms<T, N>(P, dq, M, g, cdq, K);
-  K.sync();
+// The tail of plant_step once M, g and C dq of the state are known (M is overwritten by its Cholesky factor): the
+// applied torque, the semi-implicit Euler update of q and dq, and the cost increment of the control point x.
+template <typename T, int N>
+ABRB_HD void plant_advance(T (*M)[N], const T *g, const T *cdq, T *q, T *dq, const T *u, bool comp_g, const T *x,
+                           const T *p, T dt, T effort, T *tau, T &cost) {
+  T Mi[N], rhs[N];
   chol<T, N>(M, Mi);
   ABRB_UNROLL
   for (int k = 0; k < N; ++k) {
@@ -201,6 +204,25 @@ ABRB_HD void plant_step(const ChainK<T, N> &P, int frame, const T *xoff, T *q, T
   ABRB_UNROLL
   for (int k = 0; k < N; ++k) eu += tau[k] * tau[k];
   cost += ex + effort * eu;
+}
+
+// One step of the open-loop plant rollout (plant_kernel), for the torque row `u` and the path row `p` (3 values used,
+// or nullptr):
+//     tau = u, or u - g with comp_g (the residual-torque form);  x = control point (frame + xoff) at q
+//     ddq = M^-1 (tau + g - C dq);  dq += ddq dt;  q += dq dt
+//     cost += |x - p[:3]|^2 (with a path) + effort |tau|^2
+// `tau` and `x` belong to the state BEFORE the update, as in rollout_step.
+template <typename T, int N, class K_>
+ABRB_HD void plant_step(const ChainK<T, N> &P, int frame, const T *xoff, T *q, T *dq, const T *u, bool comp_g,
+                        const T *p, T dt, T effort, T *tau, T *x, T &cost, K_ &K) {
+  K.sync();
+  walk<T, N>(P, q, frame, K);
+  K.sync();
+  frame_point(K.F, xoff, x);
+  T M[N][N], g[N], cdq[N];
+  plant_terms<T, N>(P, dq, M, g, cdq, K);
+  K.sync();
+  plant_advance<T, N>(M, g, cdq, q, dq, u, comp_g, x, p, dt, effort, tau, cost);
 }
 
 }  // namespace abrb

@@ -1154,4 +1154,121 @@ int abrb_plant_rollout_f32(const abrb_model *m, int frame_id, const double *x_of
                        effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream, true);
 }
 
+
+// ------------------------------------------------------------------------------------------------ plant derivatives
+static int dynamics_derivatives(const abrb_model *m, const void *q, const void *dq, const void *in, void *d_q,
+                                void *d_dq, void *d_in, int64_t B, void *stream, bool f32, int kind) {
+  const char *who = kind == 0 ? "abrb_forward_dynamics_derivatives" : "abrb_inverse_dynamics_derivatives";
+  const char *in_name = kind == 0 ? "u" : "ddq", *d_in_name = kind == 0 ? "d_u" : "d_ddq";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (B == 0) return ABRB_OK;
+  const void *ptrs[] = {q, dq, in, d_q, d_dq};
+  const char *names[] = {"q", "dq", in_name, "d_q", "d_dq"};
+  for (int i = 0; i < 5; ++i) {
+    if (!ptrs[i]) return fail(ABRB_EINVAL, w + ": NULL " + names[i]);
+    if (!aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  }
+  if (d_in && !aligned_elem(d_in, f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + d_in_name + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  DynJacCall k{kind, q, dq, in, d_q, d_dq, d_in, B, f32, (cudaStream_t)stream};
+  int e = cudaErrorInvalidValue;
+  switch (m->host.n) {
+#define X(j) case j: e = launch_dyn_jac<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_forward_dynamics_derivatives_f64(const abrb_model *m, const double *q, const double *dq, const double *u,
+                                          double *d_q, double *d_dq, double *d_u, int64_t B, void *stream) {
+  return dynamics_derivatives(m, q, dq, u, d_q, d_dq, d_u, B, stream, false, 0);
+}
+int abrb_forward_dynamics_derivatives_f32(const abrb_model *m, const float *q, const float *dq, const float *u,
+                                          float *d_q, float *d_dq, float *d_u, int64_t B, void *stream) {
+  return dynamics_derivatives(m, q, dq, u, d_q, d_dq, d_u, B, stream, true, 0);
+}
+int abrb_inverse_dynamics_derivatives_f64(const abrb_model *m, const double *q, const double *dq, const double *ddq,
+                                          double *d_q, double *d_dq, double *d_ddq, int64_t B, void *stream) {
+  return dynamics_derivatives(m, q, dq, ddq, d_q, d_dq, d_ddq, B, stream, false, 1);
+}
+int abrb_inverse_dynamics_derivatives_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq,
+                                          float *d_q, float *d_dq, float *d_ddq, int64_t B, void *stream) {
+  return dynamics_derivatives(m, q, dq, ddq, d_q, d_dq, d_ddq, B, stream, true, 1);
+}
+
+static int plant_rollout_vjp(const abrb_model *m, int frame_id, const double *x_off, const void *q0, const void *dq0,
+                             const void *u, int u_stride, int compensate_gravity, const void *path, int path_stride,
+                             int steps, double dt, double effort_weight, const void *q_traj, const void *dq_traj,
+                             const void *g_cost, const void *g_q, const void *g_dq, const void *g_q_traj,
+                             const void *g_dq_traj, const void *g_u_traj, const void *g_x_traj, void *gu, void *gq0,
+                             void *gdq0, int64_t B, void *stream, bool f32) {
+  const char *who = "abrb_plant_rollout_vjp";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (steps < 0) return fail(ABRB_EINVAL, w + ": steps < 0");
+  const int n = m->host.n;
+  if (frame_id < 0 || frame_id > 2 * n + 1) return fail(ABRB_EFRAME, w + ": invalid frame id");
+  if (u_stride != 0 && u_stride != n) return fail(ABRB_EINVAL, w + ": u_stride must be 0 or n_joints");
+  if (path_stride != 0 && path_stride != 6) return fail(ABRB_EINVAL, w + ": path_stride must be 0 or 6");
+  if (!std::isfinite(effort_weight) || effort_weight < 0.0)
+    return fail(ABRB_EINVAL, w + ": effort_weight must be finite and >= 0");
+  if (B == 0) return ABRB_OK;
+  if (!q0) return fail(ABRB_EINVAL, w + ": NULL q0");
+  if (!dq0) return fail(ABRB_EINVAL, w + ": NULL dq0");
+  if (!gq0) return fail(ABRB_EINVAL, w + ": NULL gq0");
+  if (!gdq0) return fail(ABRB_EINVAL, w + ": NULL gdq0");
+  if (steps > 0) {
+    if (!u) return fail(ABRB_EINVAL, w + ": NULL u");
+    if (!q_traj) return fail(ABRB_EINVAL, w + ": NULL q_traj");
+    if (!dq_traj) return fail(ABRB_EINVAL, w + ": NULL dq_traj");
+    if (!gu) return fail(ABRB_EINVAL, w + ": NULL gu");
+  }
+  const void *ptrs[] = {q0, dq0, u, path, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj,
+                        gu, gq0, gdq0};
+  const char *names[] = {"q0", "dq0", "u", "path", "q_traj", "dq_traj", "g_cost", "g_q", "g_dq", "g_q_traj",
+                         "g_dq_traj", "g_u_traj", "g_x_traj", "gu", "gq0", "gdq0"};
+  for (int i = 0; i < 16; ++i)
+    if (ptrs[i] && !aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  PlantVjpCall k{frame_id, x_off, q0, dq0, u, u_stride, compensate_gravity, path, path_stride, steps, dt,
+                 effort_weight, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj,
+                 gu, gq0, gdq0, B, f32, (cudaStream_t)stream};
+  int e = cudaErrorInvalidValue;
+  switch (n) {
+#define X(j) case j: e = launch_plant_vjp<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_plant_rollout_vjp_f64(const abrb_model *m, int frame_id, const double *x_off, const double *q0,
+                               const double *dq0, const double *u, int u_stride, int compensate_gravity,
+                               const double *path, int path_stride, int steps, double dt, double effort_weight,
+                               const double *q_traj, const double *dq_traj, const double *g_cost, const double *g_q,
+                               const double *g_dq, const double *g_q_traj, const double *g_dq_traj,
+                               const double *g_u_traj, const double *g_x_traj, double *gu, double *gq0, double *gdq0,
+                               int64_t B, void *stream) {
+  return plant_rollout_vjp(m, frame_id, x_off, q0, dq0, u, u_stride, compensate_gravity, path, path_stride, steps, dt,
+                           effort_weight, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj,
+                           gu, gq0, gdq0, B, stream, false);
+}
+int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *x_off, const float *q0,
+                               const float *dq0, const float *u, int u_stride, int compensate_gravity,
+                               const float *path, int path_stride, int steps, double dt, double effort_weight,
+                               const float *q_traj, const float *dq_traj, const float *g_cost, const float *g_q,
+                               const float *g_dq, const float *g_q_traj, const float *g_dq_traj,
+                               const float *g_u_traj, const float *g_x_traj, float *gu, float *gq0, float *gdq0,
+                               int64_t B, void *stream) {
+  return plant_rollout_vjp(m, frame_id, x_off, q0, dq0, u, u_stride, compensate_gravity, path, path_stride, steps, dt,
+                           effort_weight, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj,
+                           gu, gq0, gdq0, B, stream, true);
+}
+
 }  // extern "C"

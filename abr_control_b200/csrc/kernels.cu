@@ -12,6 +12,7 @@
 #include <atomic>
 
 #include "abrb_coop.cuh"
+#include "abrb_grad.cuh"
 #include "abrb_launch.hpp"
 #include "abrb_osc.cuh"
 #include "abrb_rbd.cuh"
@@ -693,6 +694,137 @@ dyn_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ DynAr
   }
 }
 
+// ------------------------------------------------------------------------------------------------ derivatives
+// The derivative kernels run one warp per state (dyn_jac_kernel) or per trajectory (plant_vjp_kernel); lane j < 3N
+// pushes direction j of the inputs through one dual evaluation (abrb_grad.cuh), and the other lanes idle.  The dual
+// kinematic scratch (16 B a slot in fp64) lives in shared memory, one column per working lane (stride 3N); CTAs are
+// 128 threads for orthonormal chains and 64 for general frames, whose scratch is 21 N slots instead of 9 N.
+template <bool ORTHO>
+struct DualBlock {
+  static constexpr int value = ORTHO ? 128 : 64;
+};
+template <typename T, int N, bool ORTHO>
+struct DualSmem {
+  static constexpr size_t kWarpBytes = (size_t)3 * N * KinSlots<N, ORTHO>::kCount * sizeof(Dual<T>);
+  static constexpr size_t kBytes = kWarpBytes * (DualBlock<ORTHO>::value / 32);
+};
+
+template <typename T, int N, bool ORTHO>
+__device__ __forceinline__ void bind_dual_kin(Kin<Dual<T>, N, ORTHO, StridedStore> &K, unsigned char *smem, int warp,
+                                              int lane) {
+  K.s.base = reinterpret_cast<Dual<T> *>(smem + warp * DualSmem<T, N, ORTHO>::kWarpBytes) + lane;
+  K.s.stride = 3 * N;
+}
+
+template <typename T>
+struct DynJacArgs {
+  const T *q, *dq, *in;
+  T *d_q, *d_dq, *d_in;
+  int64_t B;
+  int kind;
+};
+
+// abrb_{forward,inverse}_dynamics_derivatives_*: lane j writes column j of the state's three n x n blocks, so each
+// store instruction of a warp covers whole contiguous rows of a block
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(DualBlock<ORTHO>::value)
+dyn_jac_kernel(const __grid_constant__ ChainK<Dual<T>, N> P, const __grid_constant__ DynJacArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  constexpr int kW = DualBlock<ORTHO>::value / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  Kin<Dual<T>, N, ORTHO, StridedStore> K;
+  bind_dual_kin<T, N, ORTHO>(K, smem_raw, warp, lane);
+  const int ncol = a.d_in != nullptr ? 3 * N : 2 * N;
+  for (int64_t b = (int64_t)blockIdx.x * kW + warp; b < a.B; b += (int64_t)gridDim.x * kW) {
+    if (lane >= ncol) continue;
+    T q[N], dq[N], in[N], col[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      q[k] = a.q[b * N + k];
+      dq[k] = a.dq[b * N + k];
+      in[k] = a.in[b * N + k];
+    }
+    dyn_jac_column<T, N>(P, a.kind, lane, q, dq, in, col, K);
+    T *dst = lane < N ? a.d_q : (lane < 2 * N ? a.d_dq : a.d_in);
+    const int c = lane < N ? lane : (lane < 2 * N ? lane - N : lane - 2 * N);
+#pragma unroll
+    for (int i = 0; i < N; ++i) dst[(b * N + i) * N + c] = col[i];
+  }
+}
+
+template <typename T>
+struct PlantVjpArgs {
+  const T *q0, *dq0, *u, *path, *q_traj, *dq_traj;
+  const T *g_cost, *g_q, *g_dq, *g_q_traj, *g_dq_traj, *g_u_traj, *g_x_traj;
+  T *gu, *gq0, *gdq0;
+  int64_t B;
+  int u_stride, path_stride, steps, frame, comp_g;
+  T dt, effort;
+  T xoff[3];
+};
+
+// abrb_plant_rollout_vjp_*: the adjoint recursion of the rollout, t = S-1 .. 0, one warp per trajectory.  Every lane
+// holds mu (the cotangent of x_{t+1}); lane j < 3N computes its entry of lambda_t (j < 2N) or of the torque cotangent
+// (j >= 2N, stored), and lambda_t is broadcast with shuffles as the next step's mu.  No per-step Jacobian is stored.
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(DualBlock<ORTHO>::value)
+plant_vjp_kernel(const __grid_constant__ ChainK<Dual<T>, N> P, const __grid_constant__ PlantVjpArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  constexpr int kW = DualBlock<ORTHO>::value / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  Kin<Dual<T>, N, ORTHO, StridedStore> K;
+  bind_dual_kin<T, N, ORTHO>(K, smem_raw, warp, lane);
+  const Dual<T> xo[3] = {Dual<T>(a.xoff[0]), Dual<T>(a.xoff[1]), Dual<T>(a.xoff[2])};
+  for (int64_t b = (int64_t)blockIdx.x * kW + warp; b < a.B; b += (int64_t)gridDim.x * kW) {
+    T mu[2 * N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      mu[k] = a.g_q != nullptr ? a.g_q[b * N + k] : T(0);
+      mu[N + k] = a.g_dq != nullptr ? a.g_dq[b * N + k] : T(0);
+    }
+    const T gc = a.g_cost != nullptr ? a.g_cost[b] : T(0);
+    for (int t = a.steps - 1; t >= 0; --t) {
+      const int64_t row = (int64_t)t * a.B + b;
+      if (a.g_q_traj != nullptr) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) mu[k] += a.g_q_traj[row * N + k];
+      }
+      if (a.g_dq_traj != nullptr) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) mu[N + k] += a.g_dq_traj[row * N + k];
+      }
+      T val = T(0);
+      if (lane < 3 * N) {
+        const T *qs = t > 0 ? a.q_traj + (row - a.B) * N : a.q0 + b * N;
+        const T *dqs = t > 0 ? a.dq_traj + (row - a.B) * N : a.dq0 + b * N;
+        T q[N], dq[N], ur[N], pr[3];
+        const T *ut = torque_row<T, N>(a.u, a.u_stride, t, a.B, b);
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+          q[k] = qs[k];
+          dq[k] = dqs[k];
+          ur[k] = ut[k];
+        }
+        if (a.path != nullptr) {
+          const T *pt = path_row(a.path, a.path_stride, t, a.B, b);
+#pragma unroll
+          for (int c = 0; c < 3; ++c) pr[c] = pt[c];
+        }
+        val = plant_vjp_lane<T, N>(P, a.frame, xo, lane, q, dq, ur, a.comp_g != 0, a.path != nullptr ? pr : nullptr,
+                                   a.dt, a.effort, mu, gc, a.g_x_traj != nullptr ? a.g_x_traj + row * 3 : nullptr,
+                                   a.g_u_traj != nullptr ? a.g_u_traj + row * N : nullptr, K);
+        if (lane >= 2 * N) a.gu[row * N + lane - 2 * N] = val;
+      }
+#pragma unroll
+      for (int k = 0; k < 2 * N; ++k) mu[k] = __shfl_sync(0xffffffffu, val, k);
+    }
+    if (lane < N)
+      a.gq0[b * N + lane] = mu[lane];
+    else if (lane < 2 * N)
+      a.gdq0[b * N + lane - N] = mu[lane];
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ launch
 // kernel<<<grid, block, smem, stream>>>(args...) with programmatic stream serialization allowed: the launch may be
 // brought onto the SMs while the stream's previous kernel drains; the kernels launched through it (osc_kernel,
@@ -1104,6 +1236,83 @@ template <>
 int launch_dyn<ABRB_N>(const ChainHost &h, const DynCall &c) {
   if (c.f32) return h.ortho ? dyn_go<float, ABRB_N, true>(h, c) : dyn_go<float, ABRB_N, false>(h, c);
   return h.ortho ? dyn_go<double, ABRB_N, true>(h, c) : dyn_go<double, ABRB_N, false>(h, c);
+}
+
+template <typename T, int N, bool ORTHO>
+int dyn_jac_go(const ChainHost &h, const DynJacCall &c) {
+  ChainK<Dual<T>, N> P;
+  fill_chain<Dual<T>, N>(h, P);
+  DynJacArgs<T> a;
+  a.q = static_cast<const T *>(c.q);
+  a.dq = static_cast<const T *>(c.dq);
+  a.in = static_cast<const T *>(c.in);
+  a.d_q = static_cast<T *>(c.d_q);
+  a.d_dq = static_cast<T *>(c.d_dq);
+  a.d_in = static_cast<T *>(c.d_in);
+  a.B = c.B;
+  a.kind = c.kind;
+  constexpr int kW = DualBlock<ORTHO>::value / 32;
+  const size_t smem = DualSmem<T, N, ORTHO>::kBytes;
+  auto kern = dyn_jac_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  const int64_t blocks = (c.B + kW - 1) / kW, cap = (int64_t)num_sms() * 16;
+  kern<<<(unsigned)(blocks < cap ? blocks : cap), DualBlock<ORTHO>::value, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO>
+int plant_vjp_go(const ChainHost &h, const PlantVjpCall &c) {
+  ChainK<Dual<T>, N> P;
+  fill_chain<Dual<T>, N>(h, P);
+  PlantVjpArgs<T> a;
+  a.q0 = static_cast<const T *>(c.q0);
+  a.dq0 = static_cast<const T *>(c.dq0);
+  a.u = static_cast<const T *>(c.u);
+  a.path = static_cast<const T *>(c.path);
+  a.q_traj = static_cast<const T *>(c.q_traj);
+  a.dq_traj = static_cast<const T *>(c.dq_traj);
+  a.g_cost = static_cast<const T *>(c.g_cost);
+  a.g_q = static_cast<const T *>(c.g_q);
+  a.g_dq = static_cast<const T *>(c.g_dq);
+  a.g_q_traj = static_cast<const T *>(c.g_q_traj);
+  a.g_dq_traj = static_cast<const T *>(c.g_dq_traj);
+  a.g_u_traj = static_cast<const T *>(c.g_u_traj);
+  a.g_x_traj = static_cast<const T *>(c.g_x_traj);
+  a.gu = static_cast<T *>(c.gu);
+  a.gq0 = static_cast<T *>(c.gq0);
+  a.gdq0 = static_cast<T *>(c.gdq0);
+  a.B = c.B;
+  a.u_stride = c.u_stride;
+  a.path_stride = c.path_stride;
+  a.steps = c.steps;
+  a.frame = c.frame;
+  a.comp_g = c.compensate_gravity;
+  a.dt = T(c.dt);
+  a.effort = T(c.effort_weight);
+  for (int i = 0; i < 3; ++i) a.xoff[i] = c.xoff ? T(c.xoff[i]) : T(0);
+  constexpr int kW = DualBlock<ORTHO>::value / 32;
+  const size_t smem = DualSmem<T, N, ORTHO>::kBytes;
+  auto kern = plant_vjp_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  const int64_t blocks = (c.B + kW - 1) / kW, cap = (int64_t)num_sms() * 16;
+  kern<<<(unsigned)(blocks < cap ? blocks : cap), DualBlock<ORTHO>::value, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <>
+int launch_dyn_jac<ABRB_N>(const ChainHost &h, const DynJacCall &c) {
+  if (c.f32) return h.ortho ? dyn_jac_go<float, ABRB_N, true>(h, c) : dyn_jac_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? dyn_jac_go<double, ABRB_N, true>(h, c) : dyn_jac_go<double, ABRB_N, false>(h, c);
+}
+
+template <>
+int launch_plant_vjp<ABRB_N>(const ChainHost &h, const PlantVjpCall &c) {
+  if (c.f32) return h.ortho ? plant_vjp_go<float, ABRB_N, true>(h, c) : plant_vjp_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? plant_vjp_go<double, ABRB_N, true>(h, c) : plant_vjp_go<double, ABRB_N, false>(h, c);
 }
 
 template <>

@@ -375,6 +375,52 @@ int abrb_plant_rollout_f32(const abrb_model *m, int frame_id, const double *x_of
                            float *q_traj, float *dq_traj, float *u_traj, float *x_traj, float *cost,
                            int64_t B, void *stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Derivatives of the plant (forward-mode dual numbers through the same per-state code, DESIGN.md S3.6).
+ * Every derivative is (B, n, n) row-major, element [b, i, j] = d out_i / d in_j:
+ *   forward:  d_q = d ddq / d q,  d_dq = d ddq / d dq,  d_u = d ddq / d u = M^-1   (d_u may be NULL)
+ *   inverse:  d_q = d u / d q,    d_dq = d u / d dq,    d_ddq = d u / d ddq = M    (d_ddq may be NULL)
+ * B == 0 does nothing.  ABRB_EINVAL: NULL model or required array, B < 0, misaligned pointers.
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_forward_dynamics_derivatives_f64(const abrb_model *m, const double *q, const double *dq, const double *u,
+                                          double *d_q, double *d_dq, double *d_u, int64_t B, void *stream);
+int abrb_forward_dynamics_derivatives_f32(const abrb_model *m, const float *q, const float *dq, const float *u,
+                                          float *d_q, float *d_dq, float *d_u, int64_t B, void *stream);
+int abrb_inverse_dynamics_derivatives_f64(const abrb_model *m, const double *q, const double *dq, const double *ddq,
+                                          double *d_q, double *d_dq, double *d_ddq, int64_t B, void *stream);
+int abrb_inverse_dynamics_derivatives_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq,
+                                          float *d_q, float *d_dq, float *d_ddq, int64_t B, void *stream);
+
+/* Vector-Jacobian product of abrb_plant_rollout_*: given the rollout's arguments (q0, dq0: the START state), the
+ * states it recorded (q_traj, dq_traj: (steps, B, n), required when steps > 0) and cotangents of its outputs, each
+ * NULL (zero) or
+ *     g_cost (B),  g_q, g_dq (B,n) of the final state,  g_q_traj, g_dq_traj, g_u_traj (steps, B, n),  g_x_traj
+ *     (steps, B, 3)
+ * writes the cotangents gu (steps, B, n) of the torques — per trajectory also for a shared (u_stride 0) sequence,
+ * whose gradient is their sum over B — and gq0, gdq0 (B,n) of the start state.  Backward recursion over
+ * t = S-1 .. 0 with mu_S = (g_q, g_dq), x_t = (q_t, dq_t) the state before step t and Phi_t the step:
+ *     mu_{t+1} += (g_q_traj[t], g_dq_traj[t])
+ *     lambda_t  = g_cost dc_t/dx_t + g_x_traj[t] dx_t/dx_t + g_u_traj[t] dtau_t/dx_t + (dPhi_t/dx_t)^T mu_{t+1}
+ *     gu[t]     = g_cost dc_t/du_t + g_u_traj[t] dtau_t/du_t + (dPhi_t/du_t)^T mu_{t+1};     mu_t = lambda_t
+ * and (gq0, gdq0) = lambda_0 (= (g_q, g_dq) for steps == 0).  The path, dt and effort_weight are constants.
+ * Argument errors as abrb_plant_rollout_*, plus NULL q0, dq0, gq0, gdq0, and (steps > 0) NULL u, q_traj, dq_traj,
+ * gu: ABRB_EINVAL.
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_plant_rollout_vjp_f64(const abrb_model *m, int frame_id, const double *x_off, const double *q0,
+                               const double *dq0, const double *u, int u_stride, int compensate_gravity,
+                               const double *path, int path_stride, int steps, double dt, double effort_weight,
+                               const double *q_traj, const double *dq_traj, const double *g_cost, const double *g_q,
+                               const double *g_dq, const double *g_q_traj, const double *g_dq_traj,
+                               const double *g_u_traj, const double *g_x_traj, double *gu, double *gq0, double *gdq0,
+                               int64_t B, void *stream);
+int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *x_off, const float *q0,
+                               const float *dq0, const float *u, int u_stride, int compensate_gravity,
+                               const float *path, int path_stride, int steps, double dt, double effort_weight,
+                               const float *q_traj, const float *dq_traj, const float *g_cost, const float *g_q,
+                               const float *g_dq, const float *g_q_traj, const float *g_dq_traj,
+                               const float *g_u_traj, const float *g_x_traj, float *gu, float *gq0, float *gdq0,
+                               int64_t B, void *stream);
+
 /* Kernel launch counter for this process (every launch of a libabrb kernel increments it). */
 int64_t abrb_launch_count(void);
 
