@@ -40,6 +40,12 @@ _djac = [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
 # m, frame_id, x_off, q0, dq0, u, u_stride, compensate_gravity, path, path_stride, steps, dt, effort_weight,
 # q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj, gu, gq0, gdq0, B, stream
 _vjp = [_VP, _I, _VP, _VP, _VP, _VP, _I, _I, _VP, _I, _I, _D, _D] + [_VP] * 12 + [_I64, _VP]
+# m, kp, kv, account_for_gravity, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride, steps, dt,
+# effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream
+_joint_roll = [_VP, _D, _D, _I, _I, _VP, _VP, _VP, _VP, _I, _VP, _I, _I, _D, _D, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
+# m, kd, lamb, cartesian, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride, path_acc, pa_stride,
+# steps, dt, effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream
+_sliding_roll = _joint_roll[:12] + [_VP, _I] + _joint_roll[12:]
 SIGNATURES = {
     "abrb_version": (_I, []),
     "abrb_last_error": (_CP, []),
@@ -98,6 +104,10 @@ SIGNATURES = {
     "abrb_inverse_dynamics_derivatives_f32": (_I, _djac),
     "abrb_plant_rollout_vjp_f64": (_I, _vjp),
     "abrb_plant_rollout_vjp_f32": (_I, _vjp),
+    "abrb_joint_rollout_path_f64": (_I, _joint_roll),
+    "abrb_joint_rollout_path_f32": (_I, _joint_roll),
+    "abrb_sliding_rollout_path_f64": (_I, _sliding_roll),
+    "abrb_sliding_rollout_path_f32": (_I, _sliding_roll),
     "abrb_launch_count": (_I64, []),
 }
 

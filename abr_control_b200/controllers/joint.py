@@ -60,3 +60,36 @@ class Joint(Controller):
                     u.data_ptr(), B)
 
         return _device_call(rc, L.abrb_joint_generate_f32, L.abrb_joint_generate_f64, args, [qa, dqa, tgt, tv], single)
+
+    def rollout_path(self, q, dq, path, dt=1e-3, path_velocity=None, ref_frame="EE", xyz_offset=None,
+                     record=("q", "dq", "u", "x"), effort_weight=0.0):
+        """Closed-loop rollout of this controller along a joint-space path on the GPU (include/abrb.h,
+        abrb_joint_rollout_path_*): for each step ``t = 0 .. S-1``::
+
+            u_t = generate(q_t, dq_t, target=path[t], target_velocity=path_velocity[t])
+            x_t = Tx(ref_frame, q_t, x=xyz_offset)
+            ddq = M^-1 (u_t + g - C dq_t);  dq_{t+1} = dq_t + ddq dt;  q_{t+1} = q_t + dq_{t+1} dt
+            cost += |wrap(path[t] - q_t)|^2 + effort_weight * |u_t|^2        (wrap: into [-pi, pi), as generate)
+
+        ``path`` and ``path_velocity`` (rad/s; None: zero) are ``(S, n)`` (shared by every trajectory) or ``(S, B,
+        n)``.  Returns ``(q_final, dq_final, traj, cost)`` as ``OSC.rollout_path``: ``traj[k]`` for k in ``record`` is
+        ``(S, B, n)`` (``"x"``: ``(S, B, 3)``); ``traj["u"][t]`` and ``traj["x"][t]`` belong to the state before step
+        t, ``traj["q"][t]`` and ``traj["dq"][t]`` to the state after it; ``cost`` is ``(B,)``; ``record=()`` gives the
+        final state and the cost only.  CUDA tensors in -> CUDA tensors out; NumPy in -> NumPy out; a single state
+        ``(n,)`` takes an ``(S, n)`` path and returns ``(S, .)`` records and a scalar cost.  ``q`` and ``dq`` are not
+        modified.  The plant is that of ``simulate``, so ``traj["u"]`` replayed there gives back the track.
+
+        Tracking joint paths planned by ``InverseKinematics.generate_path`` for a batch of starts: its ``(B, S, n)``
+        position path is a view of one ``(S, B, n)`` buffer, so ``permute`` hands it over without a copy.  The
+        planner's velocity path is the joint step of each iteration, not a velocity in rad/s, so it is not a
+        ``path_velocity``::
+
+            pos, _ = ik.generate_path(q0, targets, n_timesteps=S)          # (B, S, n)
+            qf, dqf, tr, cost = Joint(rc, kp=300, kv=20).rollout_path(q0, dq0, pos.permute(1, 0, 2))
+        """
+        rc = self.robot_config
+        n = rc.N_JOINTS
+        gains = (float(self.kp), float(self.kv), int(bool(self.account_for_gravity)))
+        return _batch.ctrl_rollout(rc, ("abrb_joint_rollout_path_f64", "abrb_joint_rollout_path_f32"), gains, q, dq,
+                                   [(path, "path"), (path_velocity, "path_velocity")], n, dt, ref_frame, xyz_offset,
+                                   record, effort_weight, "rollout_path")

@@ -64,3 +64,33 @@ class Sliding(Controller):
             return np.array(u[0], dtype=np.float64) if single else u
         self.s = s[0] if single else s
         return u[0] if single else u
+
+    def rollout_path(self, q, dq, path, dt=1e-3, path_velocity=None, path_acc=None, ref_frame="EE", offset=None,
+                     record=("q", "dq", "u", "x"), effort_weight=0.0):
+        """Closed-loop rollout of this controller along a path on the GPU (include/abrb.h,
+        abrb_sliding_rollout_path_*): for each step ``t = 0 .. S-1``::
+
+            u_t = generate(q_t, dq_t, path[t], path_velocity[t], path_acc[t], ref_frame, offset)
+            x_t = Tx(ref_frame, q_t, x=offset)
+            ddq = M^-1 (u_t + g - C dq_t);  dq_{t+1} = dq_t + ddq dt;  q_{t+1} = q_t + dq_{t+1} dt
+            cost += e_t + effort_weight * |u_t|^2
+
+        with the error the controller drives to zero: ``e_t = |x_t - path[t]|^2`` in Cartesian mode and
+        ``|q_t - path[t]|^2`` (not wrapped, as the reference's joint-mode error) in joint mode, where ``ref_frame``
+        and ``offset`` only choose the recorded ``x``.  ``path``, ``path_velocity`` and ``path_acc`` (None: zero) have
+        rows of 3 values (Cartesian) or n (joint mode), ``(S, w)`` shared by every trajectory or ``(S, B, w)``.
+
+        Gravity: ``generate`` adds ``+g`` as the reference does (sliding.py:97), while the plant is held still by
+        ``u = -g``; so on an arm with gravity the closed loop runs against a ``2 g`` bias.  The rollout reproduces
+        ``generate`` as it is.
+
+        Returns ``(q_final, dq_final, traj, cost)`` as ``OSC.rollout_path`` (records ``"q"``, ``"dq"``, ``"u"``:
+        ``(S, B, n)``, ``"x"``: ``(S, B, 3)``; ``u`` and ``x`` of the state before step t, ``q`` and ``dq`` after it;
+        ``record=()`` for the cost only), in the input's form (CUDA tensors or NumPy; a single ``(n,)`` state takes an
+        ``(S, w)`` path).  ``q``, ``dq`` and ``self.s`` are left as they are."""
+        rc = self.robot_config
+        w = 3 if self.cartesian else rc.N_JOINTS
+        gains = (float(self.kd), float(self.lamb), int(bool(self.cartesian)))
+        return _batch.ctrl_rollout(rc, ("abrb_sliding_rollout_path_f64", "abrb_sliding_rollout_path_f32"), gains, q,
+                                   dq, [(path, "path"), (path_velocity, "path_velocity"), (path_acc, "path_acc")], w,
+                                   dt, ref_frame, offset, record, effort_weight, "rollout_path")

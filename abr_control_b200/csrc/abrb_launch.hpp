@@ -129,6 +129,26 @@ struct PlantCall {
   cudaStream_t stream;
 };
 
+// abrb_joint_rollout_path_* (kind kCtrlJoint) and abrb_sliding_rollout_path_* (kCtrlSliding): closed-loop rollouts
+struct CtrlRolloutCall {
+  int kind;
+  double kp, kv;  // Joint
+  int gravity;
+  double kd, lamb;  // Sliding
+  int cartesian;
+  int frame;
+  const double *xoff;           // host, 3 values or nullptr
+  void *q, *dq;                 // device, in/out
+  const void *path, *pv, *pa;   // (steps, B, w) for stride w, (steps, w) for 0; pv, pa may be nullptr
+  int path_stride, pv_stride, pa_stride;
+  int steps;
+  double dt, effort_weight;
+  void *q_traj, *dq_traj, *u_traj, *x_traj, *cost;  // each nullptr or device
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+
 // abrb_forward_dynamics_* (kind 0: in = u, out = ddq) and abrb_inverse_dynamics_* (kind 1: in = ddq, out = u)
 struct DynCall {
   int kind;
@@ -181,6 +201,7 @@ template <int N> int launch_sliding(const ChainHost &h, const SlidingCall &c);
 template <int N> int launch_ik(const ChainHost &h, const IkCall &c);
 template <int N> int launch_plant(const ChainHost &h, const PlantCall &c);
 template <int N> int launch_dyn(const ChainHost &h, const DynCall &c);
+template <int N> int launch_ctrl_rollout(const ChainHost &h, const CtrlRolloutCall &c);
 template <int N> int launch_dyn_jac(const ChainHost &h, const DynJacCall &c);
 template <int N> int launch_plant_vjp(const ChainHost &h, const PlantVjpCall &c);
 

@@ -4,6 +4,7 @@
 // damping.py:21-32, resting_config.py:25-42 + joint.py:104-131, avoid_obstacles.py:38-120.
 #pragma once
 #include "abrb_math.cuh"
+#include "abrb_rbd.cuh"
 
 namespace abrb {
 
@@ -914,6 +915,88 @@ ABRB_HD void sliding_state(const ChainK<T, N> &P, T kd, T lamb, bool cartesian, 
     if (s_out != nullptr) s_out[a] = sa;
     u[a] = acc + g[a] - kd * sa;
   }
+}
+
+// ------------------------------------------------------------------------------------------------ Joint / Sliding rollouts
+// The closed-loop rollouts of the trajectory-tracking controllers other than OSC (ctrl_rollout_kernel): the controller
+// (joint_state / sliding_state) and the plant (plant_step) as they are, one after the other, each with its own walk.
+// KIND is compile-time because the two live sets differ widely (Sliding carries J, dJ, C and RowPinv3).
+enum { kCtrlJoint = 0, kCtrlSliding = 1 };
+
+template <typename T>
+struct CtrlK {
+  T kp, kv;       // Joint
+  T kd, lamb;     // Sliding
+  int gravity;    // Joint: account_for_gravity
+  int cartesian;  // Sliding: task-space target (rows of 3) or joint-space target (rows of N)
+};
+
+// Width of the path rows of a ctrl rollout, and the length of the arrays they are loaded into (>= 3, so that a
+// cartesian row fits whatever N is)
+template <int N>
+struct CtrlRow {
+  static constexpr int kMax = N > 3 ? N : 3;
+};
+
+// Row t of trajectory b of one of a ctrl rollout's path arrays, addressed by torque_row<T, W> ((steps, B, W) for stride
+// W, one (steps, W) row sequence for stride 0), copied into `out` and padded with zeros; nullptr gives a zero row.
+template <typename T, int W, int LEN>
+ABRB_HD void ctrl_row(const T *a, int stride, int t, int64_t B, int64_t b, T *out) {
+  const T *r = a != nullptr ? torque_row<T, W>(a, stride, t, B, b) : nullptr;
+  ABRB_UNROLL
+  for (int k = 0; k < LEN; ++k) out[k] = (r != nullptr && k < W) ? r[k] : T(0);
+}
+
+// Path, path velocity and path acceleration rows of step t: width 3 for cartesian Sliding, N otherwise
+template <typename T, int N, int KIND>
+ABRB_HD void ctrl_path_rows(const T *path, int ps, const T *pv, int pvs, const T *pa, int pas, bool cartesian, int t,
+                            int64_t B, int64_t b, T *tg, T *tv, T *ta) {
+  constexpr int L = CtrlRow<N>::kMax;
+  if (KIND == kCtrlSliding && cartesian) {
+    ctrl_row<T, 3, L>(path, ps, t, B, b, tg);
+    ctrl_row<T, 3, L>(pv, pvs, t, B, b, tv);
+    ctrl_row<T, 3, L>(pa, pas, t, B, b, ta);
+  } else {
+    ctrl_row<T, N, L>(path, ps, t, B, b, tg);
+    ctrl_row<T, N, L>(pv, pvs, t, B, b, tv);
+    if (KIND == kCtrlSliding) ctrl_row<T, N, L>(pa, pas, t, B, b, ta);
+  }
+}
+
+// One step of the Joint / Sliding rollouts, for the path rows `target`, `tv` and `ta` (tv, ta nullptr: zero):
+//     u = Joint.generate(q, dq, target, tv)   or   Sliding.generate(q, dq, target, tv, ta, frame, xoff)
+//     x = control point (frame + xoff) at q;  ddq = M^-1 (u + g - C dq);  dq += ddq dt;  q += dq dt
+//     cost += e + effort |u|^2,  e = |wrap(target - q)|^2 (Joint), |x - target|^2 (cartesian Sliding),
+//                                    |q - target|^2 (joint-mode Sliding: not wrapped, as in the reference)
+// `u`, `x` and e belong to the state BEFORE the update, as in rollout_step and plant_step.
+template <typename T, int N, int KIND, class K_>
+ABRB_HD void ctrl_rollout_step(const ChainK<T, N> &P, const CtrlK<T> &G, int frame, const T *xoff, T *q, T *dq,
+                               const T *target, const T *tv, const T *ta, T dt, T effort, T *u, T *x, T &cost,
+                               K_ &K) {
+  K.sync();
+  if (KIND == kCtrlJoint)
+    joint_state<T, N>(P, G.kp, G.kv, G.gravity != 0, q, dq, target, tv, u, K);
+  else
+    sliding_state<T, N>(P, G.kd, G.lamb, G.cartesian != 0, frame, xoff, q, dq, target, tv, ta, u, (T *)nullptr, K);
+  const bool task = KIND == kCtrlSliding && G.cartesian != 0;
+  T e = T(0);
+  if (!task) {
+    ABRB_UNROLL
+    for (int k = 0; k < N; ++k) {
+      const T d = KIND == kCtrlJoint ? wrap_pm_pi(target[k] - q[k]) : q[k] - target[k];
+      e += d * d;
+    }
+  }
+  T tau[N];
+  plant_step<T, N>(P, frame, xoff, q, dq, u, false, (const T *)nullptr, dt, effort, tau, x, cost, K);
+  if (task) {
+    ABRB_UNROLL
+    for (int c = 0; c < 3; ++c) {
+      const T d = x[c] - target[c];
+      e += d * d;
+    }
+  }
+  cost += e;
 }
 
 // One iteration of InverseKinematics.generate_path (controllers/path_planners/inverse_kinematics.py:83-137): the joint

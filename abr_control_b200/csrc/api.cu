@@ -1154,6 +1154,107 @@ int abrb_plant_rollout_f32(const abrb_model *m, int frame_id, const double *x_of
                        effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream, true);
 }
 
+// ------------------------------------------------------------------------------------------------ Joint / Sliding rollouts
+// `k` carries the controller (kind, gains, flags), the frame and the records; its path strides are checked here against
+// the row width w (3 for cartesian Sliding, n_joints otherwise)
+static int ctrl_rollout(const abrb_model *m, CtrlRolloutCall k, const char *who) {
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (k.B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (k.steps < 0) return fail(ABRB_EINVAL, w + ": steps < 0");
+  const int n = m->host.n;
+  if (k.frame < 0 || k.frame > 2 * n + 1) return fail(ABRB_EFRAME, w + ": invalid frame id");
+  const bool task = k.kind == kCtrlSliding && k.cartesian;
+  const int width = task ? 3 : n;
+  const char *wname = task ? "3 (cartesian)" : "n_joints";
+  const int strides[] = {k.path_stride, k.pv_stride, k.pa_stride};
+  const char *snames[] = {"path_stride", "pv_stride", "pa_stride"};
+  for (int i = 0; i < (k.kind == kCtrlSliding ? 3 : 2); ++i)
+    if (strides[i] != 0 && strides[i] != width) return fail(ABRB_EINVAL, w + ": " + snames[i] + " must be 0 or " + wname);
+  if (!std::isfinite(k.effort_weight) || k.effort_weight < 0.0)
+    return fail(ABRB_EINVAL, w + ": effort_weight must be finite and >= 0");
+  if (k.B == 0) return ABRB_OK;
+  if (!k.q) return fail(ABRB_EINVAL, w + ": NULL q");
+  if (!k.dq) return fail(ABRB_EINVAL, w + ": NULL dq");
+  if (k.steps > 0 && !k.path) return fail(ABRB_EINVAL, w + ": NULL path");
+  const void *ptrs[] = {k.q, k.dq, k.path, k.pv, k.pa, k.q_traj, k.dq_traj, k.u_traj, k.x_traj, k.cost};
+  const char *names[] = {"q", "dq", "path", "path_velocity", "path_acc", "q_traj", "dq_traj", "u_traj", "x_traj",
+                         "cost"};
+  for (int i = 0; i < 10; ++i)
+    if (ptrs[i] && !aligned_elem(ptrs[i], k.f32))
+      return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  if (k.steps == 0) {  // nothing to step: q and dq stay as they are, the cost is zero
+    int e = k.cost ? (int)cudaMemsetAsync(k.cost, 0, (size_t)k.B * (k.f32 ? 4 : 8), k.stream) : 0;
+    return e ? cuda_fail(e, who) : ABRB_OK;
+  }
+  int e = cudaErrorInvalidValue;
+  switch (n) {
+#define X(j) case j: e = launch_ctrl_rollout<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+static int joint_rollout(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                         const double *x_off, void *q, void *dq, const void *path, int path_stride,
+                         const void *path_velocity, int pv_stride, int steps, double dt, double effort_weight,
+                         void *q_traj, void *dq_traj, void *u_traj, void *x_traj, void *cost, int64_t B, void *stream,
+                         bool f32) {
+  CtrlRolloutCall k{kCtrlJoint, kp, kv, account_for_gravity, 0.0, 0.0, 0, frame_id, x_off, q, dq, path,
+                    path_velocity, nullptr, path_stride, pv_stride, 0, steps, dt, effort_weight, q_traj, dq_traj,
+                    u_traj, x_traj, cost, B, f32, (cudaStream_t)stream};
+  return ctrl_rollout(m, k, "abrb_joint_rollout_path");
+}
+
+static int sliding_rollout(const abrb_model *m, double kd, double lamb, int cartesian, int frame_id,
+                           const double *x_off, void *q, void *dq, const void *path, int path_stride,
+                           const void *path_velocity, int pv_stride, const void *path_acc, int pa_stride, int steps,
+                           double dt, double effort_weight, void *q_traj, void *dq_traj, void *u_traj, void *x_traj,
+                           void *cost, int64_t B, void *stream, bool f32) {
+  CtrlRolloutCall k{kCtrlSliding, 0.0, 0.0, 0, kd, lamb, cartesian != 0, frame_id, x_off, q, dq, path, path_velocity,
+                    path_acc, path_stride, pv_stride, pa_stride, steps, dt, effort_weight, q_traj, dq_traj, u_traj,
+                    x_traj, cost, B, f32, (cudaStream_t)stream};
+  return ctrl_rollout(m, k, "abrb_sliding_rollout_path");
+}
+
+int abrb_joint_rollout_path_f64(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                const double *x_off, double *q, double *dq, const double *path, int path_stride,
+                                const double *path_velocity, int pv_stride, int steps, double dt,
+                                double effort_weight, double *q_traj, double *dq_traj, double *u_traj,
+                                double *x_traj, double *cost, int64_t B, void *stream) {
+  return joint_rollout(m, kp, kv, account_for_gravity, frame_id, x_off, q, dq, path, path_stride, path_velocity,
+                       pv_stride, steps, dt, effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream, false);
+}
+int abrb_joint_rollout_path_f32(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                const double *x_off, float *q, float *dq, const float *path, int path_stride,
+                                const float *path_velocity, int pv_stride, int steps, double dt, double effort_weight,
+                                float *q_traj, float *dq_traj, float *u_traj, float *x_traj, float *cost, int64_t B,
+                                void *stream) {
+  return joint_rollout(m, kp, kv, account_for_gravity, frame_id, x_off, q, dq, path, path_stride, path_velocity,
+                       pv_stride, steps, dt, effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B, stream, true);
+}
+int abrb_sliding_rollout_path_f64(const abrb_model *m, double kd, double lamb, int cartesian, int frame_id,
+                                  const double *x_off, double *q, double *dq, const double *path, int path_stride,
+                                  const double *path_velocity, int pv_stride, const double *path_acc, int pa_stride,
+                                  int steps, double dt, double effort_weight, double *q_traj, double *dq_traj,
+                                  double *u_traj, double *x_traj, double *cost, int64_t B, void *stream) {
+  return sliding_rollout(m, kd, lamb, cartesian, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride,
+                         path_acc, pa_stride, steps, dt, effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B,
+                         stream, false);
+}
+int abrb_sliding_rollout_path_f32(const abrb_model *m, double kd, double lamb, int cartesian, int frame_id,
+                                  const double *x_off, float *q, float *dq, const float *path, int path_stride,
+                                  const float *path_velocity, int pv_stride, const float *path_acc, int pa_stride,
+                                  int steps, double dt, double effort_weight, float *q_traj, float *dq_traj,
+                                  float *u_traj, float *x_traj, float *cost, int64_t B, void *stream) {
+  return sliding_rollout(m, kd, lamb, cartesian, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride,
+                         path_acc, pa_stride, steps, dt, effort_weight, q_traj, dq_traj, u_traj, x_traj, cost, B,
+                         stream, true);
+}
+
 
 // ------------------------------------------------------------------------------------------------ plant derivatives
 static int dynamics_derivatives(const abrb_model *m, const void *q, const void *dq, const void *in, void *d_q,

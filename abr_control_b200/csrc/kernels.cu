@@ -654,6 +654,65 @@ plant_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ Pla
 }
 
 template <typename T>
+struct CtrlRolloutArgs {
+  T *q, *dq;
+  const T *path, *pv, *pa;  // rows of width 3 (cartesian Sliding) or N at torque_row(.., stride, t, B, b); pv, pa may be
+                            // nullptr (pa: Sliding only)
+  T *q_traj, *dq_traj, *u_traj, *x_traj, *cost;
+  int64_t B;
+  int path_stride, pv_stride, pa_stride, steps, frame;
+  CtrlK<T> G;
+  T dt, effort;
+  T xoff[3];
+};
+
+// Closed-loop Joint / Sliding rollout (abrb_joint_rollout_path_*, abrb_sliding_rollout_path_*): one trajectory per
+// thread, q and dq in registers across the steps, the controller and the plant of each step in ctrl_rollout_step
+// (abrb_osc.cuh).  Shaped like plant_kernel, with the same kinematic scratch.
+template <typename T, int N, bool ORTHO, int KIND>
+__global__ void __launch_bounds__(kBlock)
+ctrl_rollout_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ CtrlRolloutArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef WarpSmem<T, N, ORTHO, (N > 3 ? N : 3)> WS;
+  constexpr int L = CtrlRow<N>::kMax;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
+  T *stage = region + WS::kKin;
+  typename KS::type K;
+  KS::bind(K, region, lane);
+  for (int64_t base = (int64_t)blockIdx.x * kBlock; base < a.B; base += (int64_t)gridDim.x * kBlock) {
+    const int64_t warp_b0 = base + warp * 32;
+    if (warp_b0 >= a.B) break;
+    const int64_t rem = a.B - warp_b0;
+    const int nvalid = rem < 32 ? (int)rem : 32;
+    const int64_t b = warp_b0 + (lane < nvalid ? lane : nvalid - 1);
+    T q[N], dq[N], tg[L], tv[L], ta[L], u[N], x[3];
+    T cost = T(0);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      q[k] = a.q[b * N + k];
+      dq[k] = a.dq[b * N + k];
+    }
+    for (int t = 0; t < a.steps; ++t) {
+      // a shared path is one address for the whole warp (a broadcast load), a per-trajectory one a row per lane
+      ctrl_path_rows<T, N, KIND>(a.path, a.path_stride, a.pv, a.pv_stride, a.pa, a.pa_stride, a.G.cartesian != 0, t,
+                                 a.B, b, tg, tv, ta);
+      ctrl_rollout_step<T, N, KIND>(P, a.G, a.frame, a.xoff, q, dq, tg, a.pv != nullptr ? tv : nullptr,
+                                    a.pa != nullptr ? ta : nullptr, a.dt, a.effort, u, x, cost, K);
+      const int64_t row0 = (int64_t)t * a.B + warp_b0;
+      if (a.u_traj) store_records<T, N>(a.u_traj, row0, nvalid, u, stage, lane);
+      if (a.q_traj) store_records<T, N>(a.q_traj, row0, nvalid, q, stage, lane);
+      if (a.dq_traj) store_records<T, N>(a.dq_traj, row0, nvalid, dq, stage, lane);
+      if (a.x_traj) store_records<T, 3>(a.x_traj, row0, nvalid, x, stage, lane);
+    }
+    store_records<T, N>(a.q, warp_b0, nvalid, q, stage, lane);
+    store_records<T, N>(a.dq, warp_b0, nvalid, dq, stage, lane);
+    if (a.cost != nullptr && lane < nvalid) a.cost[b] = cost;
+  }
+}
+
+template <typename T>
 struct DynArgs {
   const T *q, *dq, *in;  // in: u (kind 0) or ddq (kind 1)
   T *out;                // ddq (kind 0) or u (kind 1)
@@ -1230,6 +1289,57 @@ template <>
 int launch_plant<ABRB_N>(const ChainHost &h, const PlantCall &c) {
   if (c.f32) return h.ortho ? plant_go<float, ABRB_N, true>(h, c) : plant_go<float, ABRB_N, false>(h, c);
   return h.ortho ? plant_go<double, ABRB_N, true>(h, c) : plant_go<double, ABRB_N, false>(h, c);
+}
+
+template <typename T, int N, bool ORTHO, int KIND>
+int ctrl_rollout_go(const ChainHost &h, const CtrlRolloutCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  CtrlRolloutArgs<T> a;
+  a.q = static_cast<T *>(c.q);
+  a.dq = static_cast<T *>(c.dq);
+  a.path = static_cast<const T *>(c.path);
+  a.pv = static_cast<const T *>(c.pv);
+  a.pa = static_cast<const T *>(c.pa);
+  a.q_traj = static_cast<T *>(c.q_traj);
+  a.dq_traj = static_cast<T *>(c.dq_traj);
+  a.u_traj = static_cast<T *>(c.u_traj);
+  a.x_traj = static_cast<T *>(c.x_traj);
+  a.cost = static_cast<T *>(c.cost);
+  a.B = c.B;
+  a.path_stride = c.path_stride;
+  a.pv_stride = c.pv_stride;
+  a.pa_stride = c.pa_stride;
+  a.steps = c.steps;
+  a.frame = c.frame;
+  a.G.kp = T(c.kp);
+  a.G.kv = T(c.kv);
+  a.G.kd = T(c.kd);
+  a.G.lamb = T(c.lamb);
+  a.G.gravity = c.gravity;
+  a.G.cartesian = c.cartesian;
+  a.dt = T(c.dt);
+  a.effort = T(c.effort_weight);
+  for (int i = 0; i < 3; ++i) a.xoff[i] = c.xoff ? T(c.xoff[i]) : T(0);
+  const size_t smem = (size_t)kWarps * WarpSmem<T, N, ORTHO, (N > 3 ? N : 3)>::kElems * sizeof(T);
+  auto kern = ctrl_rollout_kernel<T, N, ORTHO, KIND>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <typename T, int KIND>
+int ctrl_rollout_ortho(const ChainHost &h, const CtrlRolloutCall &c) {
+  return h.ortho ? ctrl_rollout_go<T, ABRB_N, true, KIND>(h, c) : ctrl_rollout_go<T, ABRB_N, false, KIND>(h, c);
+}
+
+template <>
+int launch_ctrl_rollout<ABRB_N>(const ChainHost &h, const CtrlRolloutCall &c) {
+  if (c.kind == kCtrlJoint)
+    return c.f32 ? ctrl_rollout_ortho<float, kCtrlJoint>(h, c) : ctrl_rollout_ortho<double, kCtrlJoint>(h, c);
+  return c.f32 ? ctrl_rollout_ortho<float, kCtrlSliding>(h, c) : ctrl_rollout_ortho<double, kCtrlSliding>(h, c);
 }
 
 template <>

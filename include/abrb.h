@@ -456,6 +456,53 @@ int abrb_ik_path_f32(const abrb_model *m, double max_dx, double max_dr, double m
                      int n_timesteps, const float *position, const float *target, int target_stride,
                      float *position_path, float *velocity_path, int64_t B, void *stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Closed-loop rollouts of Joint and Sliding along a path, the counterpart of abrb_osc_rollout_path_* for the other
+ * trajectory-tracking controllers.  For t = 0 .. steps-1, from the state (q_t, dq_t) before the step:
+ *     u_t      = Joint.generate(q_t, dq_t, path_t, path_velocity_t)      (as abrb_joint_generate_*)
+ *     u_t      = Sliding.generate(q_t, dq_t, path_t, path_velocity_t, path_acc_t, frame_id, x_off)
+ *                                                                          (as abrb_sliding_generate_*)
+ *     x_t      = position of the control point (frame_id + x_off) at q_t
+ *     ddq_t    = M(q_t)^-1 (u_t + g(q_t) - C(q_t, dq_t) dq_t)
+ *     dq_{t+1} = dq_t + ddq_t dt;   q_{t+1} = q_t + dq_{t+1} dt
+ *     cost    += e_t + effort_weight |u_t|^2,   e_t = |wrap_pm_pi(path_t - q_t)|^2   (Joint)
+ *                                               e_t = |x_t - path_t|^2             (Sliding, cartesian != 0)
+ *                                               e_t = |q_t - path_t|^2             (Sliding, joint mode; not wrapped)
+ * The plant is that of abrb_plant_rollout_*, so u_traj replayed there (no path, same effort_weight) gives back q, dq
+ * and x.  Sliding keeps the reference's +g (sliding.py:97): with gravity the closed loop runs against a 2 g bias.
+ * Records as abrb_plant_rollout_*: x_traj[t] and u_traj[t] belong to the state BEFORE step t, q_traj[t] and
+ * dq_traj[t] to the state AFTER it.  In joint-mode Sliding, frame_id and x_off only choose the recorded x.
+ *   q, dq          (B,n) in/out (final state)
+ *   path, path_velocity, path_acc: rows of width w = 3 (cartesian Sliding) or n; stride w: (steps, B, w), element
+ *                  (t, b, k) at [(t*B + b)*w + k]; stride 0: one (steps, w) sequence for every trajectory.
+ *                  path_velocity and path_acc may be NULL (zero).
+ *   q_traj / dq_traj / u_traj: NULL or (steps, B, n);   x_traj: NULL or (steps, B, 3);   cost: NULL or (B,)
+ *   effort_weight  finite, >= 0 (double for both precisions, as dt, the gains and x_off)
+ * steps == 0 leaves q, dq unchanged and writes cost = 0; B == 0 does nothing.  Arguments are checked before any
+ * device work: ABRB_EINVAL (NULL model, q, dq, or path when steps > 0; a stride other than 0 or w; negative steps or
+ * B; effort_weight negative or not finite; misaligned pointers), ABRB_EFRAME (bad frame id).
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_joint_rollout_path_f64(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                const double *x_off, double *q, double *dq, const double *path, int path_stride,
+                                const double *path_velocity, int pv_stride, int steps, double dt,
+                                double effort_weight, double *q_traj, double *dq_traj, double *u_traj,
+                                double *x_traj, double *cost, int64_t B, void *stream);
+int abrb_joint_rollout_path_f32(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                const double *x_off, float *q, float *dq, const float *path, int path_stride,
+                                const float *path_velocity, int pv_stride, int steps, double dt, double effort_weight,
+                                float *q_traj, float *dq_traj, float *u_traj, float *x_traj, float *cost, int64_t B,
+                                void *stream);
+int abrb_sliding_rollout_path_f64(const abrb_model *m, double kd, double lamb, int cartesian, int frame_id,
+                                  const double *x_off, double *q, double *dq, const double *path, int path_stride,
+                                  const double *path_velocity, int pv_stride, const double *path_acc, int pa_stride,
+                                  int steps, double dt, double effort_weight, double *q_traj, double *dq_traj,
+                                  double *u_traj, double *x_traj, double *cost, int64_t B, void *stream);
+int abrb_sliding_rollout_path_f32(const abrb_model *m, double kd, double lamb, int cartesian, int frame_id,
+                                  const double *x_off, float *q, float *dq, const float *path, int path_stride,
+                                  const float *path_velocity, int pv_stride, const float *path_acc, int pa_stride,
+                                  int steps, double dt, double effort_weight, float *q_traj, float *dq_traj,
+                                  float *u_traj, float *x_traj, float *cost, int64_t B, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
