@@ -50,6 +50,27 @@ class NullParams(C.Structure):
     ]
 
 
+# include/abrb.h abrb_path_params / abrb_path_rec (the batched path planner)
+PATH_MAX_POINTS = 4096
+VEL_GAUSSIAN, VEL_LINEAR = 0, 1
+
+
+class PathParams(C.Structure):
+    _fields_ = [
+        ("vel_kind", C.c_int32),
+        ("n_points", C.c_int32),
+        ("dt", C.c_double),
+        ("acceleration", C.c_double),
+        ("n_sigma", C.c_double),
+        ("axes", C.c_int32 * 4),
+    ]
+
+
+class PathRec(C.Structure):
+    _fields_ = [("max_v", C.c_double), ("n_start", C.c_int32), ("n_const", C.c_int32), ("n_end", C.c_int32),
+                ("flags", C.c_int32)]
+
+
 class OscParams(C.Structure):
     _fields_ = [
         ("kp", C.c_double),

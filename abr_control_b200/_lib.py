@@ -108,6 +108,9 @@ SIGNATURES = {
     "abrb_joint_rollout_path_f32": (_I, _joint_roll),
     "abrb_sliding_rollout_path_f64": (_I, _sliding_roll),
     "abrb_sliding_rollout_path_f32": (_I, _sliding_roll),
+    "abrb_path_plan": (_I, [C.POINTER(_abi.PathParams)] + [_VP] * 8 + [_I64, _VP]),
+    "abrb_path_fill_f64": (_I, [C.POINTER(_abi.PathParams)] + [_VP] * 9 + [_I64, _VP, _I64, _VP]),
+    "abrb_path_fill_f32": (_I, [C.POINTER(_abi.PathParams)] + [_VP] * 9 + [_I64, _VP, _I64, _VP]),
     "abrb_launch_count": (_I64, []),
 }
 

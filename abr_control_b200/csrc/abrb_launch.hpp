@@ -205,6 +205,21 @@ template <int N> int launch_ctrl_rollout(const ChainHost &h, const CtrlRolloutCa
 template <int N> int launch_dyn_jac(const ChainHost &h, const DynJacCall &c);
 template <int N> int launch_plant_vjp(const ChainHost &h, const PlantVjpCall &c);
 
+// Path planner (abrb_path_*): independent of the joint count, compiled in the ABRB_N == 1 unit only.  Device arrays.
+struct PathCall {
+  abrb_path_params p;
+  const double *table, *start, *target, *max_v, *v0, *v1, *so, *to;
+  int64_t *lengths;   // phase 1 out, phase 2 in
+  abrb_path_rec *plan;
+  int64_t s_max;
+  void *path;         // phase 2 out, (s_max, B, 12 or 6)
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+int launch_path_plan(const PathCall &c);
+int launch_path_fill(const PathCall &c);
+
 void count_launch();
 
 }  // namespace abrb

@@ -1372,4 +1372,88 @@ int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *
                            gu, gq0, gdq0, B, stream, true);
 }
 
+// ------------------------------------------------------------------------------------------------ path planner
+static int path_check(const char *w, const abrb_path_params *p, const double *table, const double *start,
+                      const double *target, const void *a, const void *b, int64_t B) {
+  if (!p) return fail(ABRB_EINVAL, std::string(w) + ": NULL params");
+  if (B < 0) return fail(ABRB_EINVAL, std::string(w) + ": negative size");
+  if (p->vel_kind != ABRB_VEL_GAUSSIAN && p->vel_kind != ABRB_VEL_LINEAR)
+    return fail(ABRB_EUNSUP, std::string(w) + ": unknown velocity profile kind");
+  if (p->n_points < 2) return fail(ABRB_EINVAL, std::string(w) + ": n_points must be at least 2");
+  if (p->n_points > ABRB_PATH_MAX_POINTS)
+    return fail(ABRB_EUNSUP, std::string(w) + ": n_points above " + std::to_string(ABRB_PATH_MAX_POINTS) +
+                                 " (phase 2 keeps the warped curve in shared memory)");
+  if (p->axes[0] < 0 || p->axes[0] > 2)
+    return fail(ABRB_EUNSUP, std::string(w) + ": unknown Euler axes (first axis)");
+  for (int i = 1; i < 4; ++i)
+    if (p->axes[i] != 0 && p->axes[i] != 1) return fail(ABRB_EUNSUP, std::string(w) + ": unknown Euler axes");
+  if (!(p->dt > 0.0) || !(p->acceleration > 0.0) || !std::isfinite(p->dt) || !std::isfinite(p->acceleration) ||
+      (p->vel_kind == ABRB_VEL_GAUSSIAN && (!(p->n_sigma > 0.0) || !std::isfinite(p->n_sigma))))
+    return fail(ABRB_EINVAL, std::string(w) + ": dt, acceleration and n_sigma must be positive and finite");
+  if (B == 0) return ABRB_OK;
+  const void *ptrs[] = {table, start, target, a, b};
+  for (const void *q : ptrs) {
+    if (!q) return fail(ABRB_EINVAL, std::string(w) + ": NULL argument");
+    if (!aligned_elem(q, false)) return fail(ABRB_EINVAL, std::string(w) + ": misaligned pointer");
+  }
+  return ABRB_OK;
+}
+
+int abrb_path_plan(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                   const double *max_velocity, const double *start_velocity, const double *target_velocity,
+                   int64_t *lengths, abrb_path_rec *plan, int64_t B, void *stream) {
+  const char *w = "abrb_path_plan";
+  int rc = path_check(w, p, table, start, target, start_velocity, target_velocity, B);
+  if (rc || B == 0) return rc;
+  const void *ptrs[] = {max_velocity, lengths, plan};
+  for (const void *q : ptrs) {
+    if (!q) return fail(ABRB_EINVAL, std::string(w) + ": NULL argument");
+    if (!aligned_elem(q, false)) return fail(ABRB_EINVAL, std::string(w) + ": misaligned pointer");
+  }
+  if ((rc = ensure_device())) return rc;
+  PathCall c{*p, table, start, target, max_velocity, start_velocity, target_velocity, nullptr, nullptr, lengths, plan,
+             0, nullptr, B, false, (cudaStream_t)stream};
+  const int e = launch_path_plan(c);
+  return e ? cuda_fail(e, w) : ABRB_OK;
+}
+
+static int path_fill(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                     const double *v0, const double *v1, const double *so, const double *to, const abrb_path_rec *plan,
+                     const int64_t *lengths, int64_t s_max, void *path, int64_t B, void *stream, bool f32) {
+  const char *w = f32 ? "abrb_path_fill_f32" : "abrb_path_fill_f64";
+  int rc = path_check(w, p, table, start, target, v0, v1, B);
+  if (rc) return rc;
+  if (s_max < 0 || s_max > (int64_t(1) << 30)) return fail(ABRB_EINVAL, std::string(w) + ": s_max outside 0 .. 2^30");
+  if ((so == nullptr) != (to == nullptr))
+    return fail(ABRB_EINVAL, std::string(w) + ": give both orientations or neither");
+  if (B == 0 || s_max == 0) return ABRB_OK;
+  const void *ptrs[] = {plan, lengths, so, to};
+  for (int i = 0; i < 4; ++i) {
+    if (!ptrs[i] && i < 2) return fail(ABRB_EINVAL, std::string(w) + ": NULL argument");
+    if (ptrs[i] && !aligned_elem(ptrs[i], false)) return fail(ABRB_EINVAL, std::string(w) + ": misaligned pointer");
+  }
+  if (!path) return fail(ABRB_EINVAL, std::string(w) + ": NULL argument");
+  if (!aligned_elem(path, f32)) return fail(ABRB_EINVAL, std::string(w) + ": misaligned pointer");
+  if ((rc = ensure_device())) return rc;
+  PathCall c{*p, table, start, target, nullptr, v0, v1, so, to, const_cast<int64_t *>(lengths),
+             const_cast<abrb_path_rec *>(plan), s_max, path, B, f32, (cudaStream_t)stream};
+  const int e = launch_path_fill(c);
+  return e ? cuda_fail(e, w) : ABRB_OK;
+}
+
+int abrb_path_fill_f64(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                       const double *start_velocity, const double *target_velocity, const double *start_orientation,
+                       const double *target_orientation, const abrb_path_rec *plan, const int64_t *lengths,
+                       int64_t s_max, double *path, int64_t B, void *stream) {
+  return path_fill(p, table, start, target, start_velocity, target_velocity, start_orientation, target_orientation,
+                   plan, lengths, s_max, path, B, stream, false);
+}
+int abrb_path_fill_f32(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                       const double *start_velocity, const double *target_velocity, const double *start_orientation,
+                       const double *target_orientation, const abrb_path_rec *plan, const int64_t *lengths,
+                       int64_t s_max, float *path, int64_t B, void *stream) {
+  return path_fill(p, table, start, target, start_velocity, target_velocity, start_orientation, target_orientation,
+                   plan, lengths, s_max, path, B, stream, true);
+}
+
 }  // extern "C"

@@ -15,6 +15,7 @@
 #include "abrb_grad.cuh"
 #include "abrb_launch.hpp"
 #include "abrb_osc.cuh"
+#include "abrb_path.cuh"
 #include "abrb_rbd.cuh"
 
 #ifndef ABRB_N
@@ -1442,5 +1443,179 @@ int launch_ctrl<ABRB_N>(const ChainHost &h, const CtrlCall &c) {
   if (c.f32) return h.ortho ? ctrl_go<float, ABRB_N, true>(h, c) : ctrl_go<float, ABRB_N, false>(h, c);
   return h.ortho ? ctrl_go<double, ABRB_N, true>(h, c) : ctrl_go<double, ABRB_N, false>(h, c);
 }
+
+#if ABRB_N == 1
+// ------------------------------------------------------------------------------------------------ path planner
+// Independent of the joint count, so only the ABRB_N == 1 unit compiles it.  Both phases evaluate the planner in fp64
+// (abrb_path.cuh); phase 2 reads phase 1's record instead of repeating the search, so every row's length and segment
+// split are phase 1's by construction.
+namespace {
+
+constexpr int kPathPlanBlock = 128;  // four rows per CTA, one warp each
+constexpr int kPathBlock = 256;      // phase 2: one CTA per row
+
+// path::HostSum's order on one warp: lane l sums elements lo + l, lo + l + 32, ... then an xor butterfly.
+struct WarpSum {
+  template <class F>
+  __device__ double operator()(int lo, int n, F f) const {
+    const int lane = threadIdx.x & 31;
+    double acc = 0.0;
+    for (int i = lo + lane; i < n; i += 32) acc += f(i);
+    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    return acc;
+  }
+};
+
+__global__ void __launch_bounds__(kPathPlanBlock) path_plan_kernel(const PathCall c) {
+  const int64_t b = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (b >= c.B) return;  // warp-uniform
+  abrb_path_rec rec{0.0, 0, 0, 0, 0};
+  const int64_t len =
+      path::plan_row(c.p, c.table, c.start + 3 * b, c.target + 3 * b, c.max_v[b], c.v0[b], c.v1[b], rec, WarpSum{});
+  if ((threadIdx.x & 31) == 0) {
+    c.lengths[b] = len;
+    c.plan[b] = rec;
+  }
+}
+
+// Inclusive scan over the CTA (Hillis-Steele in each warp, then the warp totals in order).  Thread 0 gets its own x
+// back unchanged.  wsum: kPathBlock / 32 doubles of shared memory.
+__device__ double block_incl_scan(double x, double *wsum) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int off = 1; off < 32; off <<= 1) {
+    const double y = __shfl_up_sync(0xffffffffu, x, off);
+    if (lane >= off) x += y;
+  }
+  if (lane == 31) wsum[w] = x;
+  __syncthreads();
+  if (w > 0) {
+    double pre = wsum[0];
+    for (int k = 1; k < w; ++k) pre += wsum[k];
+    x = pre + x;
+  }
+  __syncthreads();
+  return x;
+}
+
+// phase 2 shared memory: arc[P], xyz[3P], path_steps window [kPathBlock + 2], warp sums [8], last row [12], p_0, p_end
+__host__ __device__ constexpr size_t path_fill_smem(int P) {
+  return sizeof(double) * (size_t(4) * P + kPathBlock + 2 + kPathBlock / 32 + 12 + 6);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kPathBlock) path_fill_kernel(const PathCall c) {
+  extern __shared__ double sm[];
+  __shared__ double carry_sh;
+  const int P = c.p.n_points, t = threadIdx.x;
+  double *arc = sm, *xyz = arc + P, *ps = xyz + 3 * P, *wsum = ps + kPathBlock + 2, *last = wsum + kPathBlock / 32,
+         *ends = last + 12;
+  const int64_t b = blockIdx.x;
+  const int w = c.so ? 12 : 6;
+  T *out = static_cast<T *>(c.path);
+  const int64_t len = c.lengths[b];
+  const int64_t S = len < c.s_max ? len : c.s_max;
+  if (S < 2) {  // a row the planner rejected: defined contents, never a path
+    for (int64_t k = t; k < c.s_max; k += kPathBlock)
+      for (int q = 0; q < w; ++q) out[(k * c.B + b) * w + q] = T(NAN);
+    return;
+  }
+  path::Frame F;
+  path::frame_of(c.start + 3 * b, c.target + 3 * b, F);
+  // dist_steps = cumsum(curve_dist_steps) and warped_xyz, chunk by chunk
+  double carry = 0.0;
+  for (int i0 = 0; i0 < P; i0 += kPathBlock) {
+    const int i = i0 + t;
+    const double s = block_incl_scan((i > 0 && i < P) ? path::seg_len(F, c.table, i) : 0.0, wsum) + carry;
+    if (i < P) {
+      arc[i] = s;
+      path::warp_point(F, c.table, i, xyz + 3 * i);
+    }
+    if (t == kPathBlock - 1) carry_sh = s;
+    __syncthreads();
+    carry = carry_sh;
+    __syncthreads();
+  }
+  const path::Profile Pr = path::profile_of(c.p, c.plan[b], c.v0[b], c.v1[b]);
+  // path_steps = cumsum(stacked * dt), one window of kPathBlock steps at a time.  Pass 0 finds p_0 and p_end (the
+  // SLERP fraction needs them at every step); pass 1 writes the rows.  Both passes compute every path_steps value with
+  // the same code, so p_end is the position of row S - 1.
+  const int passes = w == 12 ? 2 : 1;
+  double q0[4], q1[4];
+  if (w == 12) {
+    path::unit_quat(c.so + 3 * b, c.p.axes, q0);
+    path::unit_quat(c.to + 3 * b, c.p.axes, q1);
+  }
+  for (int pass = 2 - passes; pass < 2; ++pass) {
+    carry = 0.0;
+    for (int64_t k0 = 0; k0 < S; k0 += kPathBlock) {
+      const int64_t k = k0 + t;
+      const double s = block_incl_scan(k < S ? path::step_at(Pr, int(k)) : 0.0, wsum) + carry;
+      ps[t + 1] = s;
+      if (t == 0) ps[0] = carry;
+      if (t == kPathBlock - 1) ps[kPathBlock + 1] = k + 1 < S ? s + path::step_at(Pr, int(k + 1)) : 0.0;
+      if (pass == 0) {
+        if (k == 0) path::interp(arc, xyz, P, s, ends);
+        if (k == S - 1) path::interp(arc, xyz, P, s, ends + 3);
+      }
+      __syncthreads();
+      if (pass == 1 && k < S) {
+        double p[3], pm[3] = {0, 0, 0}, pp[3] = {0, 0, 0}, r[12];
+        path::interp(arc, xyz, P, s, p);
+        if (k > 0) path::interp(arc, xyz, P, ps[t], pm);
+        if (k < S - 1) path::interp(arc, xyz, P, ps[t + 2], pp);
+        for (int q = 0; q < 3; ++q) {
+          r[q] = p[q];
+          r[3 + q] = path::gradient_at(pm[q], p[q], pp[q], int(k), int(S), c.p.dt);
+        }
+        if (w == 12) {
+          double e[3], em[3] = {0, 0, 0}, ep[3] = {0, 0, 0};
+          path::orient_at(q0, q1, c.p.axes, ends, ends + 3, p, e);
+          if (k > 0) path::orient_at(q0, q1, c.p.axes, ends, ends + 3, pm, em);
+          if (k < S - 1) path::orient_at(q0, q1, c.p.axes, ends, ends + 3, pp, ep);
+          for (int q = 0; q < 3; ++q) {
+            r[6 + q] = e[q];
+            r[9 + q] = path::gradient_at(em[q], e[q], ep[q], int(k), int(S), c.p.dt);
+          }
+        }
+        T *o = out + (k * c.B + b) * w;
+        for (int q = 0; q < w; ++q) o[q] = T(r[q]);
+        if (k == S - 1)
+          for (int q = 0; q < w; ++q) last[q] = r[q];
+      }
+      carry = ps[kPathBlock];
+      __syncthreads();
+    }
+  }
+  // rows past the path repeat its last row (the reference's clamped next())
+  for (int64_t k = S + t; k < c.s_max; k += kPathBlock) {
+    T *o = out + (k * c.B + b) * w;
+    for (int q = 0; q < w; ++q) o[q] = T(last[q]);
+  }
+}
+
+}  // namespace
+
+int launch_path_plan(const PathCall &c) {
+  const int64_t grid = (c.B * 32 + kPathPlanBlock - 1) / kPathPlanBlock;
+  path_plan_kernel<<<(unsigned)grid, kPathPlanBlock, 0, c.stream>>>(c);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+int launch_path_fill(const PathCall &c) {
+  const size_t smem = path_fill_smem(c.p.n_points);
+  const void *fn = c.f32 ? (const void *)path_fill_kernel<float> : (const void *)path_fill_kernel<double>;
+  if (smem > 48 * 1024) {
+    const int e = (int)cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e) return e;
+  }
+  if (c.f32)
+    path_fill_kernel<float><<<(unsigned)c.B, kPathBlock, smem, c.stream>>>(c);
+  else
+    path_fill_kernel<double><<<(unsigned)c.B, kPathBlock, smem, c.stream>>>(c);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+#endif  // ABRB_N == 1
 
 }  // namespace abrb

@@ -503,6 +503,57 @@ int abrb_sliding_rollout_path_f32(const abrb_model *m, double kd, double lamb, i
                                   int steps, double dt, double effort_weight, float *q_traj, float *dq_traj,
                                   float *u_traj, float *x_traj, float *cost, int64_t B, void *stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Batched path planner  PathPlanner(pos_profile, vel_profile, axes).generate_path(start, target, max_velocity,
+ * start_orientation, target_orientation, start_velocity, target_velocity)  (controllers/path_planners/path_planner.py),
+ * one path per row.  The position profile enters as its table  table[i] = pos_profile.step(i / (n_points - 1)),
+ * (n_points, 3) row-major fp64 on the device; the velocity profile by kind and parameters.  All planning arithmetic is
+ * fp64 in both entry points of phase 2; only the stored rows are float in abrb_path_fill_f32.
+ *
+ * Phase 1, abrb_path_plan: per row, the warped curve's length and the reference's max_v search (starting from
+ * max_velocity, stepping down by 0.1).  lengths[b] is the row's number of steps S_b, or a negative ABRB_PATH_* reason
+ * when the reference cannot plan it; plan[b] is the record phase 2 needs.
+ * Phase 2, abrb_path_fill_*: path (s_max, B, w), w = 12 with orientations (x, dx, Euler angles, their gradient) and 6
+ * without; rows S_b .. s_max-1 repeat row S_b - 1.  Rows with lengths[b] < 2 are filled with NaN.
+ * Inputs of both phases: start, target (B,3); max_velocity, start_velocity, target_velocity (B,); orientations (B,3)
+ * Euler angles in the order params->axes.  All pointers are device pointers. */
+#define ABRB_PATH_MAX_POINTS 4096 /* n_points bound: phase 2 keeps 32 bytes per point in shared memory */
+enum { ABRB_VEL_GAUSSIAN = 0, ABRB_VEL_LINEAR = 1 };
+enum {
+  ABRB_PATH_ZERO_DISTANCE = -1, /* start == target (or a non-finite distance) */
+  ABRB_PATH_OPPOSITE = -2,      /* target - start points exactly away from (1, 1, 1): align_vectors divides by 0 */
+  ABRB_PATH_NO_VELOCITY = -3,   /* the max_v search reached 0 without fitting the ramps into the curve */
+  ABRB_PATH_SHORT_RAMP = -4,    /* a velocity ramp of fewer than two samples */
+  ABRB_PATH_TOO_LONG = -5       /* a ramp or the constant segment has 2^28 or more steps (or a non-finite count) */
+};
+typedef struct abrb_path_params {
+  int32_t vel_kind;     /* ABRB_VEL_GAUSSIAN or ABRB_VEL_LINEAR, else ABRB_EUNSUP */
+  int32_t n_points;     /* rows of table: 2 .. ABRB_PATH_MAX_POINTS (above: ABRB_EUNSUP) */
+  double dt;            /* > 0 */
+  double acceleration;  /* > 0 */
+  double n_sigma;       /* > 0, Gaussian only */
+  int32_t axes[4];      /* (firstaxis 0..2, parity, repetition, frame 0/1) of the Euler axes string, else ABRB_EUNSUP */
+} abrb_path_params;
+typedef struct abrb_path_rec {
+  double max_v;         /* the velocity the search settled on */
+  int32_t n_start, n_const, n_end;  /* samples of the starting ramp, the constant segment and the ending ramp */
+  int32_t flags;        /* bit 0: start_velocity == max_velocity (ramp [v dt]); bit 1: the same at the end */
+} abrb_path_rec;
+
+/* ABRB_EINVAL: NULL params or array, B < 0, dt / acceleration / n_sigma not > 0, n_points < 2, misaligned pointer. */
+int abrb_path_plan(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                   const double *max_velocity, const double *start_velocity, const double *target_velocity,
+                   int64_t *lengths, abrb_path_rec *plan, int64_t B, void *stream);
+/* As abrb_path_plan, and ABRB_EINVAL for s_max < 0 or above 2^30, or only one of the orientations given. */
+int abrb_path_fill_f64(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                       const double *start_velocity, const double *target_velocity, const double *start_orientation,
+                       const double *target_orientation, const abrb_path_rec *plan, const int64_t *lengths,
+                       int64_t s_max, double *path, int64_t B, void *stream);
+int abrb_path_fill_f32(const abrb_path_params *p, const double *table, const double *start, const double *target,
+                       const double *start_velocity, const double *target_velocity, const double *start_orientation,
+                       const double *target_orientation, const abrb_path_rec *plan, const int64_t *lengths,
+                       int64_t s_max, float *path, int64_t B, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
