@@ -791,9 +791,19 @@ ABRB_HD void quat_from_euler_sxyz(T ai, T aj, T ak, T *qo) {
   qo[3] = cj * cs - sj * sc;
 }
 
-// out = pinv(A) y for an R x N matrix A (row-major, R <= N expected), numpy.linalg.pinv's rcond = 1e-15: one-sided
-// Jacobi on the rows as in RowPinv3 (abrb_osc.cuh) but for any R, with every loop rolled over local-memory arrays —
-// the 15 row pairs of R = 6 unrolled would be ~3 k instructions, and this is a latency-bound sequential caller anyway.
+// Relative cut on the squared singular values of the row-Jacobi pseudo-inverses (pinv_rows_apply, RowPinv3): those at
+// or below pinv_cut2<T>() * the largest are dropped.  fp64: 1e-30, numpy.linalg.pinv's rcond = 1e-15.  fp32: 1e-12,
+// i.e. sigma <= 1e-6 sigma_max (~8 eps32): a null row of J in fp32 keeps a Jacobi residual of a few eps32 sigma_max
+// (squared ~1e-14), which 1e-30 would keep and then amplify by 1 / residual^2 (DESIGN.md, "fp32 pseudo-inverse cut").
+template <typename T>
+ABRB_HD constexpr T pinv_cut2() {
+  return sizeof(T) == 8 ? T(1e-30) : T(1e-12);
+}
+
+// out = pinv(A) y for an R x N matrix A (row-major, R <= N expected), numpy.linalg.pinv's rcond = 1e-15 in fp64
+// (pinv_cut2): one-sided Jacobi on the rows as in RowPinv3 (abrb_osc.cuh) but for any R, with every loop rolled over
+// local-memory arrays — the 15 row pairs of R = 6 unrolled would be ~3 k instructions, and this is a latency-bound
+// sequential caller anyway.
 template <typename T, int R, int N>
 ABRB_HD_NOINLINE void pinv_rows_apply(const T *A, const T *y, T *out) {
   T Bm[R][N], V[R][R];
@@ -853,7 +863,7 @@ ABRB_HD_NOINLINE void pinv_rows_apply(const T *A, const T *y, T *out) {
   for (int k = 0; k < N; ++k) out[k] = T(0);
   ABRB_NOUNROLL
   for (int i = 0; i < R; ++i) {
-    if (!(s2[i] > T(1e-30) * smax)) continue;
+    if (!(s2[i] > pinv_cut2<T>() * smax)) continue;
     T c = T(0);
     ABRB_NOUNROLL
     for (int k = 0; k < R; ++k) c += V[i][k] * y[k];

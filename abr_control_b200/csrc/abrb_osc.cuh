@@ -105,8 +105,9 @@ struct RowPinv3 {
   }
 
   // cut_rel: squared singular values <= cut_rel * largest are dropped (numpy.linalg.pinv of the 3 x N matrix with
-  // rcond = 1e-15: 1e-30; pinv(J J^T, rcond) of the symmetric product: rcond itself)
-  ABRB_HD void build(const T *r0, const T *r1, const T *r2, T cut_rel = T(1e-30)) {
+  // rcond = 1e-15: pinv_cut2, 1e-30 in fp64 and 1e-12 in fp32; pinv(J J^T, rcond) of the symmetric product: rcond
+  // itself)
+  ABRB_HD void build(const T *r0, const T *r1, const T *r2, T cut_rel = pinv_cut2<T>()) {
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) {
       b0[k] = r0[k];

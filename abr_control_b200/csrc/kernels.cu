@@ -527,17 +527,21 @@ sliding_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ S
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   T *stage = reinterpret_cast<T *>(smem_raw) + warp * kPitch * N;
   const int w = a.cartesian ? 3 : N;
+  constexpr int L = CtrlRow<N>::kMax;  // a cartesian row is 3 wide whatever N is
   for (int64_t base = (int64_t)blockIdx.x * kBlock; base < a.B; base += (int64_t)gridDim.x * kBlock) {
     const int64_t warp_b0 = base + warp * 32;
     if (warp_b0 >= a.B) break;
     const int64_t rem = a.B - warp_b0;
     const int nvalid = rem < 32 ? (int)rem : 32;
     const int64_t b = warp_b0 + (lane < nvalid ? lane : nvalid - 1);
-    T q[N], dq[N], tg[N], tv[N], ta[N], u[N], sv[N];
+    T q[N], dq[N], tg[L], tv[L], ta[L], u[N], sv[N];
 #pragma unroll
     for (int k = 0; k < N; ++k) {
       q[k] = a.q[b * N + k];
       dq[k] = a.dq[b * N + k];
+    }
+#pragma unroll
+    for (int k = 0; k < L; ++k) {
       const bool on = k < w;
       tg[k] = on ? a.target[b * a.target_stride + k] : T(0);
       tv[k] = (on && a.tv != nullptr) ? a.tv[b * a.tv_stride + k] : T(0);

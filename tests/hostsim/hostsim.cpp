@@ -103,12 +103,15 @@ void sliding_loop(const ChainHost &h, double kd, double lamb, int cartesian, int
   ChainK<T, N> P;
   fill_chain<T, N>(h, P);
   const int w = cartesian ? 3 : N;
+  constexpr int L = CtrlRow<N>::kMax;  // a cartesian row is 3 wide whatever N is
   T xo[3] = {T(xoff ? xoff[0] : 0), T(xoff ? xoff[1] : 0), T(xoff ? xoff[2] : 0)};
   for (int64_t b = 0; b < B; ++b) {
-    T qq[N], dd[N], tg[N], tvv[N], taa[N], uu[N], ss[N];
+    T qq[N], dd[N], tg[L], tvv[L], taa[L], uu[N], ss[N];
     for (int k = 0; k < N; ++k) {
       qq[k] = T(q[b * N + k]);
       dd[k] = T(dq[b * N + k]);
+    }
+    for (int k = 0; k < L; ++k) {
       tg[k] = k < w ? T(target[b * w + k]) : T(0);
       tvv[k] = (k < w && tv) ? T(tv[b * w + k]) : T(0);
       taa[k] = (k < w && ta) ? T(ta[b * w + k]) : T(0);

@@ -727,11 +727,10 @@ def test_random_chains_osc_rollout_and_controllers_on_the_device(n, dof, ortho):
     uj = Joint(rc, kp=12, kv=3).generate(q, dq, tq)
     refj = np.array([oo.Joint(oo.RobotOracle(desc), kp=12, kv=3).generate(q[i], dq[i], tq[i]) for i in range(B)])
     assert np.abs(uj - refj).max() < 1e-9 * max(1.0, np.abs(refj).max())
-    if n >= 3:
-        tg3 = rng.uniform(-0.4, 0.4, (B, 3))
-        us = Sliding(rc, kd=40.0, lamb=12.0).generate(q, dq, tg3)
-        refs, _ = oo.run_sliding_case(dict(arm=desc, ctrl=dict(kd=40.0, lamb=12.0)), q, dq, tg3, None, None)
-        assert np.max(np.abs(us - refs) / np.abs(refs).max(axis=1, keepdims=True)) < 1e-8
+    tg3 = rng.uniform(-0.4, 0.4, (B, 3))  # Cartesian rows are 3 wide whatever n is
+    us = Sliding(rc, kd=40.0, lamb=12.0).generate(q, dq, tg3)
+    refs, _ = oo.run_sliding_case(dict(arm=desc, ctrl=dict(kd=40.0, lamb=12.0)), q, dq, tg3, None, None)
+    assert np.max(np.abs(us - refs) / np.abs(refs).max(axis=1, keepdims=True)) < 1e-8
 
 
 def test_ki_integrator_vs_reference_golden():
