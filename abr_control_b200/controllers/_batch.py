@@ -11,6 +11,11 @@ def is_torch(x):
     return torch is not None and isinstance(x, torch.Tensor)
 
 
+def wants_grad(*xs):
+    """grad mode is on and one of ``xs`` is a tensor that requires grad (a differentiable rollout)"""
+    return torch is not None and torch.is_grad_enabled() and any(is_torch(x) and x.requires_grad for x in xs)
+
+
 def prep_state(rc, q, dq):
     """-> (q2, dq2, single, kind, f32) with q2/dq2 contiguous (B, n)."""
     qa, single, kind = rc._prep(q, np.float64 if (np.ndim(q) == 1 and not is_torch(q)) else None)

@@ -39,7 +39,9 @@ class Joint(Controller):
             raise NotImplementedError("ball-joint (quaternion) states are a MuJoCo-only branch of the reference")
         super().__init__(robot_config)
         self.kp = kp
-        self.kv = np.sqrt(self.kp) if kv is None else kv
+        if kv is None:  # a tensor kp keeps the default kv = sqrt(kp) in its graph
+            kv = kp.sqrt() if _batch.is_torch(kp) else np.sqrt(kp)
+        self.kv = kv
         self.account_for_gravity = account_for_gravity
         self.ZEROS_N_JOINTS = np.zeros(robot_config.N_JOINTS)
 
@@ -86,7 +88,24 @@ class Joint(Controller):
 
             pos, _ = ik.generate_path(q0, targets, n_timesteps=S)          # (B, S, n)
             qf, dqf, tr, cost = Joint(rc, kp=300, kv=20).rollout_path(q0, dq0, pos.permute(1, 0, 2))
+
+        Differentiable (``torch.autograd``, first order) when grad mode is on and ``q``, ``dq``, ``path`` or
+        ``path_velocity`` is a CUDA tensor that requires grad, or ``self.kp`` / ``self.kv`` is a 0-d CUDA tensor that
+        requires grad: gradients reach them from the cost, the final state and every returned record (``"x"``
+        included), through the adjoint recursion of ``abrb_joint_rollout_path_vjp_*``.  A shared ``(S, n)`` path or
+        velocity gets the sum over trajectories.  The wrap passes the gradient through unchanged; ``dt``,
+        ``effort_weight``, the frame and the offset are constants.  This lets a planned joint path (for instance the
+        inverse-kinematics path above) or the gains be refined so that the tracked motion improves::
+
+            path = pos.permute(1, 0, 2).clone().requires_grad_()
+            _, _, tr, _ = ctrl.rollout_path(q0, dq0, path, record=("x",))
+            ((tr["x"] - x_ref) ** 2).sum().backward()                     # path.grad: (S, B, n)
         """
+        if _batch.wants_grad(q, dq, path, path_velocity, self.kp, self.kv):
+            from . import _ctrl_autograd
+
+            return _ctrl_autograd.joint_rollout_path(self, q, dq, path, dt, path_velocity, ref_frame, xyz_offset,
+                                                     record, effort_weight)
         rc = self.robot_config
         n = rc.N_JOINTS
         gains = (float(self.kp), float(self.kv), int(bool(self.account_for_gravity)))

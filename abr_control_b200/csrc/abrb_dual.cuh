@@ -61,5 +61,11 @@ template <typename T>
 ABRB_HD Dual<T> abs_t(Dual<T> x) {
   return x.v < T(0) ? -x : x;
 }
+// fmod by a constant divisor (wrap_pm_pi): the value is the real routine's, and away from the jumps (a set of measure
+// zero) d fmod(x, y) = dx, so the tangent passes through unchanged
+template <typename T>
+ABRB_HD Dual<T> fmod_t(Dual<T> x, Dual<T> y) {
+  return Dual<T>(fmod_t(x.v, y.v), x.d);
+}
 
 }  // namespace abrb

@@ -1,6 +1,7 @@
 // abrb_grad.cuh — derivatives of the plant (DESIGN.md S3.6): one forward-mode dual evaluation per input direction.
 //
-// A lane (dyn_jac_kernel, plant_vjp_kernel) or a loop iteration (tests/hostsim/gradsim.cpp) seeds direction j of the
+// A lane (dyn_jac_kernel, plant_vjp_kernel, joint_vjp_kernel) or a loop iteration (tests/hostsim/gradsim.cpp,
+// jointgradsim.cpp) seeds direction j of the
 // inputs with a unit tangent and runs the per-state code of abrb_rbd.cuh on Dual<T>; the tangents of the outputs are
 // column j of the Jacobian.  The chain constants are a ChainK<Dual<T>, N> with zero tangents.
 //
@@ -112,6 +113,80 @@ ABRB_HD T plant_vjp_lane(const ChainK<Dual<T>, N> &P, int frame, const Dual<T> *
   if (gtau != nullptr) {
     ABRB_UNROLL
     for (int k = 0; k < N; ++k) s += gtau[k] * tau[k].d;
+  }
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) s += mu[k] * qd[k].d + mu[N + k] * dqd[k].d;
+  return s;
+}
+
+// ------------------------------------------------------------------------------------------------ the Joint closed loop
+template <typename T, int N, class K_>
+ABRB_HD_NOINLINE void phase_joint_torque(const ChainK<T, N> &P, T kp, T kv, bool gravity, const T *q, const T *dq,
+                                         const T *target, const T *tv, T *u, K_ &K) {
+  joint_torque<T, N>(P, kp, kv, gravity, q, dq, target, tv, u, K);
+}
+// The plant's tail for the Joint step: phase_advance's body in an out-of-line function of its own.  Calling
+// phase_advance from a second kernel changes the register allocation ptxas gives plant_vjp_kernel around it.
+template <typename T, int N>
+ABRB_HD_NOINLINE void phase_joint_advance(T (*M)[N], const T *g, const T *cdq, T *q, T *dq, const T *u, const T *x,
+                                          T dt, T effort, T &cost) {
+  T tau[N];
+  plant_advance<T, N>(M, g, cdq, q, dq, u, false, x, (const T *)nullptr, dt, effort, tau, cost);
+}
+
+// ctrl_rollout_step<KIND = kCtrlJoint> in phases (the same calls in the same order, each with its own walk: the
+// controller's at the base frame, the plant's at `frame`)
+template <typename T, int N, class K_>
+ABRB_HD void joint_step_phased(const ChainK<T, N> &P, T kp, T kv, bool gravity, int frame, const T *xoff, T *q, T *dq,
+                               const T *target, const T *tv, T dt, T effort, T *u, T *x, T &cost, K_ &K) {
+  phase_walk<T, N>(P, q, 0, K);
+  phase_joint_torque<T, N>(P, kp, kv, gravity, q, dq, target, tv, u, K);
+  T e = T(0);
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) {
+    const T d = wrap_pm_pi(target[k] - q[k]);
+    e += d * d;
+  }
+  phase_walk<T, N>(P, q, frame, K);
+  frame_point(K.F, xoff, x);
+  T M[N][N], g[N], cdq[N];
+  phase_terms<T, N>(P, dq, M, g, cdq, K);
+  phase_joint_advance<T, N>(M, g, cdq, q, dq, u, x, dt, effort, cost);
+  cost += e;
+}
+
+// One lane's share of the backward step t of the Joint closed loop's vector-Jacobian product (DESIGN.md S3.6).  Lane j
+// seeds one direction of (q_t, dq_t, p_t, v_t, kp, kv):
+//     j < N: q_t;  N <= j < 2N: dq_t;  2N <= j < 3N: p_t;  3N <= j < 4N: v_t;  j = 4N: kp;  j = 4N + 1: kv
+// and pushes it through one dual Joint step from the recorded state x_t = (q, dq); the result is
+//     gcost dc_t/dj + gx . dx_t/dj + gu . du_t/dj + mu . dx_{t+1}/dj
+// that is lambda_t[j] for j < 2N, the path (velocity) cotangent of step t for 2N <= j < 4N and step t's share of the
+// gain cotangent for j >= 4N.  `v` (the path velocity row) may be nullptr (zero, and lanes 3N..4N-1 then idle); gx (3)
+// and gu (N) may be nullptr (zero).
+template <typename T, int N, class K_>
+ABRB_HD T joint_vjp_lane(const ChainK<Dual<T>, N> &P, T kp, T kv, bool gravity, int frame, const Dual<T> *xoff, int j,
+                         const T *q, const T *dq, const T *p, const T *v, T dt, T effort, const T *mu, T gcost,
+                         const T *gx, const T *gu, K_ &K) {
+  typedef Dual<T> D;
+  D qd[N], dqd[N], pd[N], vd[N], u[N], x[3];
+  ABRB_UNROLL
+  for (int k = 0; k < N; ++k) {
+    qd[k] = D(q[k], unit_if<T>(j == k));
+    dqd[k] = D(dq[k], unit_if<T>(j == N + k));
+    pd[k] = D(p[k], unit_if<T>(j == 2 * N + k));
+    vd[k] = D(v != nullptr ? v[k] : T(0), unit_if<T>(j == 3 * N + k));
+  }
+  D cost = D(0);
+  joint_step_phased<D, N>(P, D(kp, unit_if<T>(j == 4 * N)), D(kv, unit_if<T>(j == 4 * N + 1)), gravity, frame, xoff, qd,
+                          dqd, pd, v != nullptr ? vd : nullptr, D(dt), D(effort), u, x, cost, K);
+  T s = gcost * cost.d;
+  if (gx != nullptr) {
+    ABRB_UNROLL
+    for (int c = 0; c < 3; ++c) s += gx[c] * x[c].d;
+  }
+  if (gu != nullptr) {
+    ABRB_UNROLL
+    for (int k = 0; k < N; ++k) s += gu[k] * u[k].d;
   }
   ABRB_UNROLL
   for (int k = 0; k < N; ++k) s += mu[k] * qd[k].d + mu[N + k] * dqd[k].d;

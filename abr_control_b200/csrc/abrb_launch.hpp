@@ -190,6 +190,26 @@ struct PlantVjpCall {
   cudaStream_t stream;
 };
 
+// abrb_joint_rollout_path_vjp_*: the Joint rollout's arguments, its recorded states and the cotangents of its outputs
+// (each nullptr or device) -> the cotangents of the path, the path velocity and the gains (each nullptr when not
+// wanted; per trajectory), q0 and dq0
+struct JointVjpCall {
+  double kp, kv;
+  int gravity;
+  int frame;
+  const double *xoff;  // host, 3 values or nullptr
+  const void *q0, *dq0, *path, *pv;
+  int path_stride, pv_stride;
+  int steps;
+  double dt, effort_weight;
+  const void *q_traj, *dq_traj;
+  const void *g_cost, *g_q, *g_dq, *g_q_traj, *g_dq_traj, *g_u_traj, *g_x_traj;
+  void *g_path, *g_pv, *g_gains, *gq0, *gdq0;
+  int64_t B;
+  bool f32;
+  cudaStream_t stream;
+};
+
 // Each returns a cudaError_t (0 = success).  Defined once per joint count in kernels.cu (-DABRB_N=<n>).
 template <int N> int launch_rbd(const ChainHost &h, const RbdCall &c);
 template <int N> int launch_osc(const ChainHost &h, const abrb_osc_params &p, const OscCall &c);
@@ -204,6 +224,7 @@ template <int N> int launch_dyn(const ChainHost &h, const DynCall &c);
 template <int N> int launch_ctrl_rollout(const ChainHost &h, const CtrlRolloutCall &c);
 template <int N> int launch_dyn_jac(const ChainHost &h, const DynJacCall &c);
 template <int N> int launch_plant_vjp(const ChainHost &h, const PlantVjpCall &c);
+template <int N> int launch_joint_vjp(const ChainHost &h, const JointVjpCall &c);
 
 // Path planner (abrb_path_*): independent of the joint count, compiled in the ABRB_N == 1 unit only.  Device arrays.
 struct PathCall {

@@ -748,11 +748,10 @@ ABRB_HD void null_state(const ChainK<T, N> &P, const NullK<T, N> &Z, const T *q,
   }
 }
 
-// Joint.generate (controllers/joint.py:104-131)
+// The tail of joint_state once the walk of q is in K: M, g and the torque
 template <typename T, int N, class K_>
-ABRB_HD void joint_state(const ChainK<T, N> &P, T kp, T kv, bool gravity, const T *q, const T *dq, const T *target,
-                         const T *tv, T *u, K_ &K) {
-  walk<T, N>(P, q, 0, K);
+ABRB_HD void joint_torque(const ChainK<T, N> &P, T kp, T kv, bool gravity, const T *q, const T *dq, const T *target,
+                          const T *tv, T *u, K_ &K) {
   T M[N][N], g[N];
   dynamics_Mg<T, N, false>(P, K, dq, M, g, nullptr);
   T w[N];
@@ -765,6 +764,14 @@ ABRB_HD void joint_state(const ChainK<T, N> &P, T kp, T kv, bool gravity, const 
     for (int b = 0; b < N; ++b) s += (b >= a ? M[a][b] : M[b][a]) * w[b];
     u[a] = gravity ? s - g[a] : s;
   }
+}
+
+// Joint.generate (controllers/joint.py:104-131)
+template <typename T, int N, class K_>
+ABRB_HD void joint_state(const ChainK<T, N> &P, T kp, T kv, bool gravity, const T *q, const T *dq, const T *target,
+                         const T *tv, T *u, K_ &K) {
+  walk<T, N>(P, q, 0, K);
+  joint_torque<T, N>(P, kp, kv, gravity, q, dq, target, tv, u, K);
 }
 
 // Floating.generate (controllers/floating.py:27-71)

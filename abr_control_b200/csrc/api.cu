@@ -1372,6 +1372,75 @@ int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *
                            gu, gq0, gdq0, B, stream, true);
 }
 
+static int joint_rollout_vjp(const abrb_model *m, JointVjpCall k) {
+  const char *who = "abrb_joint_rollout_path_vjp";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (k.B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (k.steps < 0) return fail(ABRB_EINVAL, w + ": steps < 0");
+  const int n = m->host.n;
+  if (k.frame < 0 || k.frame > 2 * n + 1) return fail(ABRB_EFRAME, w + ": invalid frame id");
+  if (k.path_stride != 0 && k.path_stride != n) return fail(ABRB_EINVAL, w + ": path_stride must be 0 or n_joints");
+  if (k.pv_stride != 0 && k.pv_stride != n) return fail(ABRB_EINVAL, w + ": pv_stride must be 0 or n_joints");
+  if (!std::isfinite(k.effort_weight) || k.effort_weight < 0.0)
+    return fail(ABRB_EINVAL, w + ": effort_weight must be finite and >= 0");
+  if (k.B == 0) return ABRB_OK;
+  if (!k.q0) return fail(ABRB_EINVAL, w + ": NULL q0");
+  if (!k.dq0) return fail(ABRB_EINVAL, w + ": NULL dq0");
+  if (!k.gq0) return fail(ABRB_EINVAL, w + ": NULL gq0");
+  if (!k.gdq0) return fail(ABRB_EINVAL, w + ": NULL gdq0");
+  if (k.steps > 0) {
+    if (!k.path) return fail(ABRB_EINVAL, w + ": NULL path");
+    if (!k.q_traj) return fail(ABRB_EINVAL, w + ": NULL q_traj");
+    if (!k.dq_traj) return fail(ABRB_EINVAL, w + ": NULL dq_traj");
+  }
+  if (k.g_pv && !k.pv) return fail(ABRB_EINVAL, w + ": g_path_velocity without path_velocity");
+  const void *ptrs[] = {k.q0, k.dq0, k.path, k.pv, k.q_traj, k.dq_traj, k.g_cost, k.g_q, k.g_dq, k.g_q_traj,
+                        k.g_dq_traj, k.g_u_traj, k.g_x_traj, k.g_path, k.g_pv, k.g_gains, k.gq0, k.gdq0};
+  const char *names[] = {"q0", "dq0", "path", "path_velocity", "q_traj", "dq_traj", "g_cost", "g_q", "g_dq",
+                         "g_q_traj", "g_dq_traj", "g_u_traj", "g_x_traj", "g_path", "g_path_velocity", "g_gains",
+                         "gq0", "gdq0"};
+  for (int i = 0; i < 18; ++i)
+    if (ptrs[i] && !aligned_elem(ptrs[i], k.f32))
+      return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  int e = cudaErrorInvalidValue;
+  switch (n) {
+#define X(j) case j: e = launch_joint_vjp<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_joint_rollout_path_vjp_f64(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                    const double *x_off, const double *q0, const double *dq0, const double *path,
+                                    int path_stride, const double *path_velocity, int pv_stride, int steps, double dt,
+                                    double effort_weight, const double *q_traj, const double *dq_traj,
+                                    const double *g_cost, const double *g_q, const double *g_dq,
+                                    const double *g_q_traj, const double *g_dq_traj, const double *g_u_traj,
+                                    const double *g_x_traj, double *g_path, double *g_path_velocity, double *g_gains,
+                                    double *gq0, double *gdq0, int64_t B, void *stream) {
+  return joint_rollout_vjp(m, {kp, kv, account_for_gravity, frame_id, x_off, q0, dq0, path, path_velocity, path_stride,
+                               pv_stride, steps, dt, effort_weight, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj,
+                               g_dq_traj, g_u_traj, g_x_traj, g_path, g_path_velocity, g_gains, gq0, gdq0, B, false,
+                               (cudaStream_t)stream});
+}
+int abrb_joint_rollout_path_vjp_f32(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                    const double *x_off, const float *q0, const float *dq0, const float *path,
+                                    int path_stride, const float *path_velocity, int pv_stride, int steps, double dt,
+                                    double effort_weight, const float *q_traj, const float *dq_traj,
+                                    const float *g_cost, const float *g_q, const float *g_dq, const float *g_q_traj,
+                                    const float *g_dq_traj, const float *g_u_traj, const float *g_x_traj,
+                                    float *g_path, float *g_path_velocity, float *g_gains, float *gq0, float *gdq0,
+                                    int64_t B, void *stream) {
+  return joint_rollout_vjp(m, {kp, kv, account_for_gravity, frame_id, x_off, q0, dq0, path, path_velocity, path_stride,
+                               pv_stride, steps, dt, effort_weight, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj,
+                               g_dq_traj, g_u_traj, g_x_traj, g_path, g_path_velocity, g_gains, gq0, gdq0, B, true,
+                               (cudaStream_t)stream});
+}
+
 // ------------------------------------------------------------------------------------------------ path planner
 static int path_check(const char *w, const abrb_path_params *p, const double *table, const double *start,
                       const double *target, const void *a, const void *b, int64_t B) {

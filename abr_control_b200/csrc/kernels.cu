@@ -889,6 +889,100 @@ plant_vjp_kernel(const __grid_constant__ ChainK<Dual<T>, N> P, const __grid_cons
   }
 }
 
+// The Joint closed loop's vector-Jacobian product has 4N + 2 working lanes (joint_vjp_lane): its dual kinematic
+// scratch is one column per working lane, (4N + 2) x KinSlots per warp, in CTAs of DualBlock<ORTHO> threads (UR5,
+// orthonormal: 22.5 KB a warp; a general 7-joint chain: 70.5 KB a warp).
+template <typename T, int N, bool ORTHO>
+struct JointDualSmem {
+  static constexpr int kCols = 4 * N + 2;
+  static constexpr size_t kWarpBytes = (size_t)kCols * KinSlots<N, ORTHO>::kCount * sizeof(Dual<T>);
+  static constexpr size_t kBytes = kWarpBytes * (DualBlock<ORTHO>::value / 32);
+};
+
+template <typename T>
+struct JointVjpArgs {
+  const T *q0, *dq0, *path, *pv, *q_traj, *dq_traj;
+  const T *g_cost, *g_q, *g_dq, *g_q_traj, *g_dq_traj, *g_u_traj, *g_x_traj;
+  T *g_path, *g_pv, *g_gains, *gq0, *gdq0;  // g_path, g_pv, g_gains may be nullptr (not wanted)
+  int64_t B;
+  int path_stride, pv_stride, steps, frame, gravity;
+  T kp, kv, dt, effort;
+  T xoff[3];
+};
+
+// abrb_joint_rollout_path_vjp_*: the adjoint recursion of the Joint closed loop, t = S-1 .. 0, one warp per trajectory,
+// shaped like plant_vjp_kernel.  Every lane holds mu; lanes j < 2N compute lambda_t, lanes 2N..4N-1 the path and path
+// velocity cotangents of step t (stored per step), lanes 4N and 4N + 1 accumulate the gain cotangents over the steps
+// (stored once).  Lanes whose output is not wanted idle.
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(DualBlock<ORTHO>::value)
+joint_vjp_kernel(const __grid_constant__ ChainK<Dual<T>, N> P, const __grid_constant__ JointVjpArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  typedef JointDualSmem<T, N, ORTHO> S;
+  constexpr int kW = DualBlock<ORTHO>::value / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  Kin<Dual<T>, N, ORTHO, StridedStore> K;
+  K.s.base = reinterpret_cast<Dual<T> *>(smem_raw + warp * S::kWarpBytes) + lane;
+  K.s.stride = S::kCols;
+  const Dual<T> xo[3] = {Dual<T>(a.xoff[0]), Dual<T>(a.xoff[1]), Dual<T>(a.xoff[2])};
+  const bool work = lane < 2 * N || (lane < 3 * N && a.g_path != nullptr) || (lane < 4 * N && lane >= 3 * N &&
+                    a.g_pv != nullptr) || (lane >= 4 * N && lane < S::kCols && a.g_gains != nullptr);
+  for (int64_t b = (int64_t)blockIdx.x * kW + warp; b < a.B; b += (int64_t)gridDim.x * kW) {
+    T mu[2 * N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      mu[k] = a.g_q != nullptr ? a.g_q[b * N + k] : T(0);
+      mu[N + k] = a.g_dq != nullptr ? a.g_dq[b * N + k] : T(0);
+    }
+    const T gc = a.g_cost != nullptr ? a.g_cost[b] : T(0);
+    T gain = T(0);
+    for (int t = a.steps - 1; t >= 0; --t) {
+      const int64_t row = (int64_t)t * a.B + b;
+      if (a.g_q_traj != nullptr) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) mu[k] += a.g_q_traj[row * N + k];
+      }
+      if (a.g_dq_traj != nullptr) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) mu[N + k] += a.g_dq_traj[row * N + k];
+      }
+      T val = T(0);
+      if (work) {
+        const T *qs = t > 0 ? a.q_traj + (row - a.B) * N : a.q0 + b * N;
+        const T *dqs = t > 0 ? a.dq_traj + (row - a.B) * N : a.dq0 + b * N;
+        const T *pt = torque_row<T, N>(a.path, a.path_stride, t, a.B, b);
+        const T *vt = a.pv != nullptr ? torque_row<T, N>(a.pv, a.pv_stride, t, a.B, b) : nullptr;
+        T q[N], dq[N], pr[N], vr[N];
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+          q[k] = qs[k];
+          dq[k] = dqs[k];
+          pr[k] = pt[k];
+          vr[k] = vt != nullptr ? vt[k] : T(0);
+        }
+        val = joint_vjp_lane<T, N>(P, a.kp, a.kv, a.gravity != 0, a.frame, xo, lane, q, dq, pr,
+                                   vt != nullptr ? vr : nullptr, a.dt, a.effort, mu, gc,
+                                   a.g_x_traj != nullptr ? a.g_x_traj + row * 3 : nullptr,
+                                   a.g_u_traj != nullptr ? a.g_u_traj + row * N : nullptr, K);
+        if (lane >= 2 * N && lane < 3 * N)
+          a.g_path[row * N + lane - 2 * N] = val;
+        else if (lane >= 3 * N && lane < 4 * N)
+          a.g_pv[row * N + lane - 3 * N] = val;
+        else if (lane >= 4 * N)
+          gain += val;
+      }
+#pragma unroll
+      for (int k = 0; k < 2 * N; ++k) mu[k] = __shfl_sync(0xffffffffu, val, k);
+    }
+    if (lane < N)
+      a.gq0[b * N + lane] = mu[lane];
+    else if (lane < 2 * N)
+      a.gdq0[b * N + lane - N] = mu[lane];
+    else if (lane >= 4 * N && lane < S::kCols && a.g_gains != nullptr)
+      a.g_gains[b * 2 + lane - 4 * N] = gain;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ launch
 // kernel<<<grid, block, smem, stream>>>(args...) with programmatic stream serialization allowed: the launch may be
 // brought onto the SMs while the stream's previous kernel drains; the kernels launched through it (osc_kernel,
@@ -1416,6 +1510,57 @@ int plant_vjp_go(const ChainHost &h, const PlantVjpCall &c) {
   kern<<<(unsigned)(blocks < cap ? blocks : cap), DualBlock<ORTHO>::value, smem, c.stream>>>(P, a);
   count_launch();
   return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO>
+int joint_vjp_go(const ChainHost &h, const JointVjpCall &c) {
+  ChainK<Dual<T>, N> P;
+  fill_chain<Dual<T>, N>(h, P);
+  JointVjpArgs<T> a;
+  a.q0 = static_cast<const T *>(c.q0);
+  a.dq0 = static_cast<const T *>(c.dq0);
+  a.path = static_cast<const T *>(c.path);
+  a.pv = static_cast<const T *>(c.pv);
+  a.q_traj = static_cast<const T *>(c.q_traj);
+  a.dq_traj = static_cast<const T *>(c.dq_traj);
+  a.g_cost = static_cast<const T *>(c.g_cost);
+  a.g_q = static_cast<const T *>(c.g_q);
+  a.g_dq = static_cast<const T *>(c.g_dq);
+  a.g_q_traj = static_cast<const T *>(c.g_q_traj);
+  a.g_dq_traj = static_cast<const T *>(c.g_dq_traj);
+  a.g_u_traj = static_cast<const T *>(c.g_u_traj);
+  a.g_x_traj = static_cast<const T *>(c.g_x_traj);
+  a.g_path = static_cast<T *>(c.g_path);
+  a.g_pv = static_cast<T *>(c.g_pv);
+  a.g_gains = static_cast<T *>(c.g_gains);
+  a.gq0 = static_cast<T *>(c.gq0);
+  a.gdq0 = static_cast<T *>(c.gdq0);
+  a.B = c.B;
+  a.path_stride = c.path_stride;
+  a.pv_stride = c.pv_stride;
+  a.steps = c.steps;
+  a.frame = c.frame;
+  a.gravity = c.gravity;
+  a.kp = T(c.kp);
+  a.kv = T(c.kv);
+  a.dt = T(c.dt);
+  a.effort = T(c.effort_weight);
+  for (int i = 0; i < 3; ++i) a.xoff[i] = c.xoff ? T(c.xoff[i]) : T(0);
+  constexpr int kW = DualBlock<ORTHO>::value / 32;
+  const size_t smem = JointDualSmem<T, N, ORTHO>::kBytes;
+  auto kern = joint_vjp_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  const int64_t blocks = (c.B + kW - 1) / kW, cap = (int64_t)num_sms() * 16;
+  kern<<<(unsigned)(blocks < cap ? blocks : cap), DualBlock<ORTHO>::value, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <>
+int launch_joint_vjp<ABRB_N>(const ChainHost &h, const JointVjpCall &c) {
+  if (c.f32) return h.ortho ? joint_vjp_go<float, ABRB_N, true>(h, c) : joint_vjp_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? joint_vjp_go<double, ABRB_N, true>(h, c) : joint_vjp_go<double, ABRB_N, false>(h, c);
 }
 
 template <>

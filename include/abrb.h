@@ -421,6 +421,42 @@ int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *
                                const float *g_u_traj, const float *g_x_traj, float *gu, float *gq0, float *gdq0,
                                int64_t B, void *stream);
 
+/* Vector-Jacobian product of abrb_joint_rollout_path_*: given the rollout's arguments (q0, dq0: the START state), the
+ * states it recorded (q_traj, dq_traj: (steps, B, n), required when steps > 0) and cotangents of its outputs, each
+ * NULL (zero) or as in abrb_plant_rollout_vjp_* (g_u_traj: of the recorded Joint torques u), writes
+ *     g_path, g_path_velocity (steps, B, n): the cotangents of the path and path velocity rows — per trajectory also
+ *         for a shared (stride 0) path, whose gradient is their sum over B; NULL: not wanted
+ *     g_gains (B, 2): [d/dkp, d/dkv] per trajectory (the gradient of the scalar gains is their sum over B); NULL: not
+ *         wanted
+ *     gq0, gdq0 (B, n): the cotangents of the start state.
+ * Backward recursion over t = S-1 .. 0 with mu_S = (g_q, g_dq), x_t = (q_t, dq_t) the state before step t, Phi_t the
+ * closed-loop step, theta_t = (path[t], path_velocity[t]) and gamma = (kp, kv):
+ *     mu_{t+1} += (g_q_traj[t], g_dq_traj[t])
+ *     lambda_t  = g_cost dc_t/dx_t + g_x_traj[t] dx^_t/dx_t + g_u_traj[t] du_t/dx_t + (dPhi_t/dx_t)^T mu_{t+1}
+ *     g_theta[t] = g_cost dc_t/dtheta_t + g_u_traj[t] du_t/dtheta_t + (dPhi_t/dtheta_t)^T mu_{t+1}
+ *     g_gamma  += g_cost dc_t/dgamma + g_u_traj[t] du_t/dgamma + (dPhi_t/dgamma)^T mu_{t+1};     mu_t = lambda_t
+ * and (gq0, gdq0) = lambda_0 (= (g_q, g_dq) and zero gains for steps == 0).  The wrap of path - q passes the tangent
+ * through unchanged; dt, effort_weight, account_for_gravity, the frame and x_off are constants.  Argument errors as
+ * abrb_joint_rollout_path_*, plus NULL q0, dq0, gq0, gdq0, (steps > 0) NULL path, q_traj, dq_traj, and a g_path_velocity
+ * without a path_velocity: ABRB_EINVAL.
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_joint_rollout_path_vjp_f64(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                    const double *x_off, const double *q0, const double *dq0, const double *path,
+                                    int path_stride, const double *path_velocity, int pv_stride, int steps, double dt,
+                                    double effort_weight, const double *q_traj, const double *dq_traj,
+                                    const double *g_cost, const double *g_q, const double *g_dq,
+                                    const double *g_q_traj, const double *g_dq_traj, const double *g_u_traj,
+                                    const double *g_x_traj, double *g_path, double *g_path_velocity, double *g_gains,
+                                    double *gq0, double *gdq0, int64_t B, void *stream);
+int abrb_joint_rollout_path_vjp_f32(const abrb_model *m, double kp, double kv, int account_for_gravity, int frame_id,
+                                    const double *x_off, const float *q0, const float *dq0, const float *path,
+                                    int path_stride, const float *path_velocity, int pv_stride, int steps, double dt,
+                                    double effort_weight, const float *q_traj, const float *dq_traj,
+                                    const float *g_cost, const float *g_q, const float *g_dq, const float *g_q_traj,
+                                    const float *g_dq_traj, const float *g_u_traj, const float *g_x_traj,
+                                    float *g_path, float *g_path_velocity, float *g_gains, float *gq0, float *gdq0,
+                                    int64_t B, void *stream);
+
 /* Kernel launch counter for this process (every launch of a libabrb kernel increments it). */
 int64_t abrb_launch_count(void);
 
