@@ -31,7 +31,7 @@ _roll = [_VP, _I, _VP, _VP, _VP, _VP, _I, _I, _D, _VP, _VP, _VP, _VP, _I64, _VP]
 # c, frame_id, x_off, q, dq, path, path_stride, path_velocity, pv_stride, steps, dt, effort_weight,
 # q_traj, dq_traj, u_traj, x_traj, cost, integrated_error, B, stream
 _roll_path = [_VP, _I, _VP, _VP, _VP, _VP, _I, _VP, _I, _I, _D, _D, _VP, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
-_dyn = [_VP, _VP, _VP, _VP, _VP, _I64, _VP]  # m, q, dq, u | ddq, ddq | u, B, stream
+_dyn = [_VP, _VP, _VP, _VP, _VP, _I64, _VP]  # m, q, dq, u | ddq, ddq | u (| Yt), B, stream
 # m, frame_id, x_off, q, dq, u, u_stride, compensate_gravity, path, path_stride, steps, dt, effort_weight,
 # q_traj, dq_traj, u_traj, x_traj, cost, B, stream
 _plant = [_VP, _I, _VP, _VP, _VP, _VP, _I, _I, _VP, _I, _I, _D, _D, _VP, _VP, _VP, _VP, _VP, _I64, _VP]
@@ -100,6 +100,8 @@ SIGNATURES = {
     "abrb_forward_dynamics_f32": (_I, _dyn),
     "abrb_inverse_dynamics_f64": (_I, _dyn),
     "abrb_inverse_dynamics_f32": (_I, _dyn),
+    "abrb_inverse_dynamics_regressor_f64": (_I, _dyn),
+    "abrb_inverse_dynamics_regressor_f32": (_I, _dyn),
     "abrb_plant_rollout_f64": (_I, _plant),
     "abrb_plant_rollout_f32": (_I, _plant),
     "abrb_forward_dynamics_derivatives_f64": (_I, _djac),

@@ -261,14 +261,19 @@ class BaseConfig:
             qa, dqa = torch.as_tensor(qa).to(dev), torch.as_tensor(dqa).to(dev)
         return qa, dqa, single, kind, f32
 
-    def _dynamics(self, q, dq, x, what, fns):
+    def _on_device_rows(self, q, dq, x, what):
+        """``_on_device`` and a third ``(B, n)`` input ``x`` of the same form -> (q, dq, x, single, kind, f32)"""
         qa, dqa, single, kind, f32 = self._on_device(q, dq)
         B, n = qa.shape
         xa = (x if _is_torch(x) else torch.as_tensor(np.asarray(x, dtype=np.float64))).to(device=qa.device,
                                                                                             dtype=qa.dtype)
         if tuple(xa.shape) != ((n,) if single else (B, n)):
             raise ValueError(f"{what} must have the shape of q, ({n},) or ({B}, {n}), got {tuple(xa.shape)}")
-        xa = xa.reshape(B, n).contiguous()
+        return qa, dqa, xa.reshape(B, n).contiguous(), single, kind, f32
+
+    def _dynamics(self, q, dq, x, what, fns):
+        qa, dqa, xa, single, kind, f32 = self._on_device_rows(q, dq, x, what)
+        B = qa.shape[0]
         out = torch.empty_like(qa)
         fn = getattr(_lib.lib(), fns[1] if f32 else fns[0])
         with torch.cuda.device(qa.device):
@@ -279,14 +284,8 @@ class BaseConfig:
         return out[0] if single else out
 
     def _derivatives(self, q, dq, x, kind, want_in=True):
-        what = "u" if kind == 0 else "ddq"
-        qa, dqa, single, hkind, f32 = self._on_device(q, dq)
+        qa, dqa, xa, single, hkind, f32 = self._on_device_rows(q, dq, x, "u" if kind == 0 else "ddq")
         B, n = qa.shape
-        xa = (x if _is_torch(x) else torch.as_tensor(np.asarray(x, dtype=np.float64))).to(device=qa.device,
-                                                                                            dtype=qa.dtype)
-        if tuple(xa.shape) != ((n,) if single else (B, n)):
-            raise ValueError(f"{what} must have the shape of q, ({n},) or ({B}, {n}), got {tuple(xa.shape)}")
-        xa = xa.reshape(B, n).contiguous()
         d = [torch.empty((B, n, n), dtype=qa.dtype, device=qa.device) for _ in range(3 if want_in else 2)]
         name = "abrb_forward_dynamics_derivatives" if kind == 0 else "abrb_inverse_dynamics_derivatives"
         fn = getattr(_lib.lib(), name + ("_f32" if f32 else "_f64"))
@@ -319,6 +318,96 @@ class BaseConfig:
 
             return _autograd.dynamics(self, 1, q, dq, ddq)
         return self._dynamics(q, dq, ddq, "ddq", ("abrb_inverse_dynamics_f64", "abrb_inverse_dynamics_f32"))
+
+    # ------------------------------------------------------------------ inertial parameters
+    def inverse_dynamics_regressor(self, q, dq, ddq):
+        """Regressor ``Y`` of ``inverse_dynamics``, linear in the inertial parameters: ``Y @ inertial_parameters() ==
+        inverse_dynamics(q, dq, ddq)`` (to rounding), column ``p = 6 (l - 1) + c`` being the torque per unit
+        ``link_inertia[l][c]`` (links 1..n; c = m_x, m_y, m_z, I_xx, I_yy, I_zz).  ``(B, n, 6n)``, or ``(n, 6n)`` for
+        one state: a view of the ``(B, 6n, n)`` record of ``abrb_inverse_dynamics_regressor_*``.  Input forms as
+        ``inverse_dynamics`` (CUDA tensors in -> CUDA tensors out, NumPy in -> NumPy out, dtype of the input)."""
+        qa, dqa, aa, single, kind, f32 = self._on_device_rows(q, dq, ddq, "ddq")
+        B, n = qa.shape
+        Yt = torch.empty((B, 6 * n, n), dtype=qa.dtype, device=qa.device)
+        L = _lib.lib()
+        fn = L.abrb_inverse_dynamics_regressor_f32 if f32 else L.abrb_inverse_dynamics_regressor_f64
+        with torch.cuda.device(qa.device):
+            _lib.check(fn(self._handle, qa.data_ptr(), dqa.data_ptr(), aa.data_ptr(), Yt.data_ptr(), B,
+                          torch.cuda.current_stream(qa.device).cuda_stream))
+        Y = Yt.cpu().numpy().transpose(0, 2, 1) if kind == "numpy" else Yt.transpose(1, 2)
+        return Y[0] if single else Y
+
+    def inertial_parameters(self):
+        """``(6n,)`` float64: this model's ``link_inertia[1:]`` flattened, the ``theta`` of
+        ``inverse_dynamics_regressor`` (link 0 never moves, so it never enters the dynamics)."""
+        return np.asarray(self.desc["link_inertia"], dtype=np.float64)[1:].reshape(-1).copy()
+
+    def with_link_inertia(self, theta):
+        """A new model with the same chain, link 0 and precision, and ``link_inertia[1:] = theta`` (``(6n,)``, as
+        ``inertial_parameters``)."""
+        n = self.N_JOINTS
+        th = np.asarray(theta.detach().cpu() if _is_torch(theta) else theta, dtype=np.float64)
+        if th.shape != (6 * n,) or not np.all(np.isfinite(th)):
+            raise ValueError(f"theta must be {6 * n} finite values, got shape {th.shape}")
+        W = np.asarray(self.desc["link_inertia"], dtype=np.float64).copy()
+        W[1:] = th.reshape(n, 6)
+        return BaseConfig(dict(self.desc, link_inertia=W.tolist()), ROBOT_NAME=self.ROBOT_NAME, dtype=self.dtype)
+
+    def identify_link_inertia(self, q, dq, ddq, u, rcond=1e-10, chunk_states=65536):
+        """Least-squares fit of the link inertias to recorded motion: the ``theta`` that minimises ``|Y theta - u|``
+        over the samples, starting from this model.  ``q, dq, ddq, u``: ``(K, n)`` samples (CUDA tensors, or NumPy
+        staged through the current device in chunks).  Returns ``(theta, info)``; ``with_link_inertia(theta)`` is the
+        identified model.
+
+        * The three mass entries of a link are one unknown (this model's must be equal), so there are 4 per link.
+        * ``G = sum Y^T Y`` and ``Y^T`` times the prior's residual are accumulated in fp64 over ``chunk_states``
+          samples at a time with the device regressor (fp32 inputs give an fp32 regressor, accumulated in fp64).
+        * Columns are equilibrated; structurally zero columns are dropped, as are eigen-directions of the equilibrated
+          Gram matrix with eigenvalue ``<= rcond * largest``.  ``theta`` is the minimum-norm update of this model's
+          parameters within the kept directions: what the data cannot see stays at the prior.
+        * ``info``: ``rank`` (kept directions), ``basis`` (``(6n, rank)``, orthonormal: the identifiable directions in
+          ``theta`` coordinates; compare models by their projections on it, not entry by entry),
+          ``unidentifiable`` (indices of ``theta`` whose column is zero), ``rms_before`` / ``rms_after`` (RMS torque
+          residual of this model and of the fit over all ``K n`` torques).
+
+        Samples from a recorded rollout (``simulate``, or a controller's ``rollout_path``) from ``(q0, dq0)`` with step
+        ``dt``: ``traj["u"][t]`` belongs to the state BEFORE step t and ``traj["q"][t]``, ``traj["dq"][t]`` to the state
+        after it, so with ``q_prev = [q0, traj["q"][:-1]]`` and ``dq_prev`` likewise, the samples are ::
+
+            q, dq = q_prev, dq_prev;  ddq = (traj["dq"] - dq_prev) / dt;  u = traj["u"]     # each (S, B, n)
+            theta, info = rc.identify_link_inertia(*(a.reshape(-1, n) for a in (q, dq, ddq, u)))
+
+        ``ddq`` is exact there (to rounding): the semi-implicit Euler step sets ``dq_{t+1} = dq_t + ddq_t dt``."""
+        from . import _ident
+
+        n = self.N_JOINTS
+        theta0 = self.inertial_parameters()
+        _ident.tied(theta0, n)
+        if chunk_states < 1:
+            raise ValueError("chunk_states must be >= 1")
+        xs = [q, dq, ddq, u]
+        on_device = all(_is_torch(x) for x in xs)
+        if on_device:
+            if not xs[0].is_cuda or any(x.device != xs[0].device or x.dtype != xs[0].dtype for x in xs):
+                raise ValueError("q, dq, ddq and u must be CUDA tensors of one device and dtype, or NumPy arrays")
+        elif any(_is_torch(x) for x in xs):
+            raise ValueError("q, dq, ddq and u must be CUDA tensors of one device and dtype, or NumPy arrays")
+        else:
+            xs = [np.asarray(x, dtype=self.dtype) for x in xs]
+        K = xs[0].shape[0] if xs[0].ndim == 2 else -1
+        if K < 1 or any(tuple(x.shape) != (K, n) for x in xs):
+            raise ValueError(f"q, dq, ddq and u must be (K, {n}) with K >= 1")
+        if on_device:
+            dev, dtype = xs[0].device, xs[0].dtype
+        else:
+            dev = torch.device("cuda", torch.cuda.current_device())
+            dtype = torch.float32 if self.dtype == np.float32 else torch.float64
+
+        def regress(i0, i1):
+            qc, dqc, ac, uc = (torch.as_tensor(x[i0:i1]).to(device=dev, dtype=dtype) for x in xs)
+            return self.inverse_dynamics_regressor(qc, dqc, ac), uc
+
+        return _ident.identify(regress, K, int(chunk_states), theta0, float(rcond))
 
     def forward_dynamics_derivatives(self, q, dq, u):
         """Derivatives of ``forward_dynamics``: ``(d_q, d_dq, d_u)``, each ``(B, n, n)`` (``(n, n)`` for one state) with

@@ -159,6 +159,16 @@ struct DynCall {
   cudaStream_t stream;
 };
 
+// abrb_inverse_dynamics_regressor_*: Yt (B, 6n, n), the transposed regressor of every state
+struct RegressorCall {
+  const void *q, *dq, *ddq;
+  void *Yt;
+  int64_t B;
+  const double *gravity;  // host, 6 values (the model's)
+  bool f32;
+  cudaStream_t stream;
+};
+
 // abrb_forward_dynamics_derivatives_* (kind 0: in = u) and abrb_inverse_dynamics_derivatives_* (kind 1: in = ddq):
 // (B, n, n) derivatives of the output with respect to q, dq and in (d_in may be nullptr)
 struct DynJacCall {
@@ -221,6 +231,7 @@ template <int N> int launch_sliding(const ChainHost &h, const SlidingCall &c);
 template <int N> int launch_ik(const ChainHost &h, const IkCall &c);
 template <int N> int launch_plant(const ChainHost &h, const PlantCall &c);
 template <int N> int launch_dyn(const ChainHost &h, const DynCall &c);
+template <int N> int launch_regressor(const ChainHost &h, const RegressorCall &c);
 template <int N> int launch_ctrl_rollout(const ChainHost &h, const CtrlRolloutCall &c);
 template <int N> int launch_dyn_jac(const ChainHost &h, const DynJacCall &c);
 template <int N> int launch_plant_vjp(const ChainHost &h, const PlantVjpCall &c);

@@ -1099,6 +1099,40 @@ int abrb_inverse_dynamics_f32(const abrb_model *m, const float *q, const float *
   return plant_dynamics(m, q, dq, ddq, u, B, stream, true, 1);
 }
 
+static int dynamics_regressor(const abrb_model *m, const void *q, const void *dq, const void *ddq, void *Yt, int64_t B,
+                              void *stream, bool f32) {
+  const char *who = "abrb_inverse_dynamics_regressor";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (B == 0) return ABRB_OK;
+  const void *ptrs[] = {q, dq, ddq, Yt};
+  const char *names[] = {"q", "dq", "ddq", "Yt"};
+  for (int i = 0; i < 4; ++i) {
+    if (!ptrs[i]) return fail(ABRB_EINVAL, w + ": NULL " + names[i]);
+    if (!aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  }
+  int rc = ensure_device();
+  if (rc) return rc;
+  RegressorCall k{q, dq, ddq, Yt, B, m->desc.gravity, f32, (cudaStream_t)stream};
+  int e = cudaErrorInvalidValue;
+  switch (m->host.n) {
+#define X(j) case j: e = launch_regressor<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_inverse_dynamics_regressor_f64(const abrb_model *m, const double *q, const double *dq, const double *ddq,
+                                        double *Yt, int64_t B, void *stream) {
+  return dynamics_regressor(m, q, dq, ddq, Yt, B, stream, false);
+}
+int abrb_inverse_dynamics_regressor_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq,
+                                        float *Yt, int64_t B, void *stream) {
+  return dynamics_regressor(m, q, dq, ddq, Yt, B, stream, true);
+}
+
 static int plant_rollout(const abrb_model *m, int frame_id, const double *x_off, void *q, void *dq, const void *u,
                          int u_stride, int compensate_gravity, const void *path, int path_stride, int steps, double dt,
                          double effort_weight, void *q_traj, void *dq_traj, void *u_traj, void *x_traj, void *cost,

@@ -17,6 +17,7 @@
 #include "abrb_osc.cuh"
 #include "abrb_path.cuh"
 #include "abrb_rbd.cuh"
+#include "abrb_regress.cuh"
 
 #ifndef ABRB_N
 #error "compile with -DABRB_N=<joint count>"
@@ -79,12 +80,13 @@ struct MaxI {
 constexpr int kPitch = 33;
 // Records longer than kChunk elements go through the tile in slices of kChunk (the tile then needs only
 // kPitch * kChunk elements per warp, which is what lets three CTAs of the fp64 kernels share an SM); each slice is a
-// run of kChunk contiguous elements per record in global memory (>= 144 bytes for fp64).
+// run of kChunk contiguous elements per record in global memory (>= 144 bytes for fp64).  STRIDE > LEN stores a part of
+// a longer record (`out` then points at the part's first element in record 0).
 constexpr int kChunk = 64;  // no slicing needed with 2 CTAs/SM (93 KB each); 18 would allow 3 CTAs/SM but measured slower
-template <typename T, int LEN>
+template <typename T, int LEN, int STRIDE = LEN>
 __device__ __forceinline__ void store_records(T *__restrict__ out, int64_t warp_b0, int nvalid, const T *rec,
                                               T *tile, int lane) {
-  T *dst = out + warp_b0 * LEN;
+  T *dst = out + warp_b0 * STRIDE;
 #pragma unroll
   for (int c0 = 0; c0 < LEN; c0 += kChunk) {
     constexpr int kFull = kChunk;
@@ -100,7 +102,7 @@ __device__ __forceinline__ void store_records(T *__restrict__ out, int64_t warp_
       if (it < ch) {
         const int i = it * 32 + lane;
         const int r = i / ch, e = i - r * ch;
-        if (i < total) dst[r * LEN + c0 + e] = tile[e * kPitch + r];
+        if (i < total) dst[r * STRIDE + c0 + e] = tile[e * kPitch + r];
       }
     }
   }
@@ -758,6 +760,60 @@ dyn_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ DynAr
   }
 }
 
+template <typename T>
+struct RegressorArgs {
+  const T *q, *dq, *ddq;
+  T *Yt;  // (B, 6N, N)
+  int64_t B;
+  T gravity[6];
+};
+
+// Output functor handed to inverse_dynamics_regressor: stores each finished half of a state's record at once
+template <typename T, int N>
+struct RegressorSink {
+  T *Yt, *tile;
+  int64_t warp_b0;
+  int nvalid, lane;
+  template <int LEN>
+  __device__ __forceinline__ void put(int off, const T *rec) {
+    store_records<T, LEN, RegressorLayout<N>::kRecord>(Yt + off, warp_b0, nvalid, rec, tile, lane);
+  }
+};
+
+// abrb_inverse_dynamics_regressor_*: one state per thread, grid-stride.  A state reads 3N values and writes 6N^2.
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(kBlock)
+regressor_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ RegressorArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  typedef KinSel<T, N, ORTHO> KS;
+  typedef WarpSmem<T, N, ORTHO, RegressorLayout<N>::kHalf> WS;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T *region = reinterpret_cast<T *>(smem_raw) + warp * WS::kElems;
+  typename KS::type K;
+  KS::bind(K, region, lane);
+  RegressorSink<T, N> sink;
+  sink.Yt = a.Yt;
+  sink.tile = region + WS::kKin;
+  sink.lane = lane;
+  for (int64_t base = (int64_t)blockIdx.x * kBlock; base < a.B; base += (int64_t)gridDim.x * kBlock) {
+    const int64_t warp_b0 = base + warp * 32;
+    if (warp_b0 >= a.B) break;
+    const int64_t rem = a.B - warp_b0;
+    const int nvalid = rem < 32 ? (int)rem : 32;
+    const int64_t b = warp_b0 + (lane < nvalid ? lane : nvalid - 1);
+    T q[N], dq[N], ddq[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      q[k] = a.q[b * N + k];
+      dq[k] = a.dq[b * N + k];
+      ddq[k] = a.ddq[b * N + k];
+    }
+    sink.warp_b0 = warp_b0;
+    sink.nvalid = nvalid;
+    inverse_dynamics_regressor<T, N>(P, a.gravity, q, dq, ddq, sink, K);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ derivatives
 // The derivative kernels run one warp per state (dyn_jac_kernel) or per trajectory (plant_vjp_kernel); lane j < 3N
 // pushes direction j of the inputs through one dual evaluation (abrb_grad.cuh), and the other lanes idle.  The dual
@@ -1384,6 +1440,26 @@ int dyn_go(const ChainHost &h, const DynCall &c) {
   return (int)cudaGetLastError();
 }
 
+template <typename T, int N, bool ORTHO>
+int regressor_go(const ChainHost &h, const RegressorCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  RegressorArgs<T> a;
+  a.q = static_cast<const T *>(c.q);
+  a.dq = static_cast<const T *>(c.dq);
+  a.ddq = static_cast<const T *>(c.ddq);
+  a.Yt = static_cast<T *>(c.Yt);
+  a.B = c.B;
+  for (int i = 0; i < 6; ++i) a.gravity[i] = T(c.gravity[i]);
+  const size_t smem = (size_t)kWarps * WarpSmem<T, N, ORTHO, RegressorLayout<N>::kHalf>::kElems * sizeof(T);
+  auto kern = regressor_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  kern<<<grid_for(c.B, 8), kBlock, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
 template <>
 int launch_plant<ABRB_N>(const ChainHost &h, const PlantCall &c) {
   if (c.f32) return h.ortho ? plant_go<float, ABRB_N, true>(h, c) : plant_go<float, ABRB_N, false>(h, c);
@@ -1445,6 +1521,12 @@ template <>
 int launch_dyn<ABRB_N>(const ChainHost &h, const DynCall &c) {
   if (c.f32) return h.ortho ? dyn_go<float, ABRB_N, true>(h, c) : dyn_go<float, ABRB_N, false>(h, c);
   return h.ortho ? dyn_go<double, ABRB_N, true>(h, c) : dyn_go<double, ABRB_N, false>(h, c);
+}
+
+template <>
+int launch_regressor<ABRB_N>(const ChainHost &h, const RegressorCall &c) {
+  if (c.f32) return h.ortho ? regressor_go<float, ABRB_N, true>(h, c) : regressor_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? regressor_go<double, ABRB_N, true>(h, c) : regressor_go<double, ABRB_N, false>(h, c);
 }
 
 template <typename T, int N, bool ORTHO>

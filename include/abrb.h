@@ -341,6 +341,21 @@ int abrb_inverse_dynamics_f64(const abrb_model *m, const double *q, const double
 int abrb_inverse_dynamics_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq,
                               float *u, int64_t B, void *stream);
 
+/* Inverse-dynamics regressor.  Inverse dynamics is linear in the diagonal link inertias:
+ *     u = M(q) ddq + C(q, dq) dq - g(q) = Y(q, dq, ddq) theta,   theta[6 (l-1) + c] = link_inertia[l][c]
+ * for links l = 1 .. n and c = 0..5 (m_x, m_y, m_z, I_xx, I_yy, I_zz); link 0 never enters.  Writes Y^T per state:
+ *   q, dq, ddq     (B,n)
+ *   Yt             (B, 6n, n), element (b, p, a) at Yt[(b*6n + p)*n + a] = d u_a / d theta_p of state b, so the 6n
+ *                  values of link l (rows 6(l-1) .. 6l-1) are contiguous in each state's record
+ * With theta the model's own constants, sum_p Yt[b, p, :] theta[p] is abrb_inverse_dynamics_* of the same state (to
+ * rounding).  The model's gravity is used.  B == 0 does nothing.  Arguments are checked before any device work:
+ * ABRB_EINVAL (NULL model or array, B < 0, misaligned pointers).
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_inverse_dynamics_regressor_f64(const abrb_model *m, const double *q, const double *dq, const double *ddq,
+                                        double *Yt, int64_t B, void *stream);
+int abrb_inverse_dynamics_regressor_f32(const abrb_model *m, const float *q, const float *dq, const float *ddq,
+                                        float *Yt, int64_t B, void *stream);
+
 /* Open-loop plant rollout under a given torque sequence u_t.  For t = 0 .. steps-1:
  *     tau_t    = u_t                       (compensate_gravity == 0)
  *     tau_t    = u_t - g(q_t)              (compensate_gravity != 0: u_t is the residual torque MPPI samples around)
