@@ -50,6 +50,9 @@ _sliding_roll = _joint_roll[:12] + [_VP, _I] + _joint_roll[12:]
 # effort_weight, q_traj, dq_traj, g_cost, g_q, g_dq, g_q_traj, g_dq_traj, g_u_traj, g_x_traj, g_path,
 # g_path_velocity, g_gains, gq0, gdq0, B, stream
 _joint_vjp = _joint_roll[:15] + [_VP] * 14 + [_I64, _VP]
+# m, q0, dq0, u, u_stride, compensate_gravity, steps, effort_weight, q_traj, dq_traj, gu, g_cost, g_u_traj, g_theta,
+# B, stream
+_theta_vjp = [_VP, _VP, _VP, _VP, _I, _I, _I, _D] + [_VP] * 6 + [_I64, _VP]
 SIGNATURES = {
     "abrb_version": (_I, []),
     "abrb_last_error": (_CP, []),
@@ -110,6 +113,8 @@ SIGNATURES = {
     "abrb_inverse_dynamics_derivatives_f32": (_I, _djac),
     "abrb_plant_rollout_vjp_f64": (_I, _vjp),
     "abrb_plant_rollout_vjp_f32": (_I, _vjp),
+    "abrb_plant_rollout_theta_vjp_f64": (_I, _theta_vjp),
+    "abrb_plant_rollout_theta_vjp_f32": (_I, _theta_vjp),
     "abrb_joint_rollout_path_f64": (_I, _joint_roll),
     "abrb_joint_rollout_path_f32": (_I, _joint_roll),
     "abrb_joint_rollout_path_vjp_f64": (_I, _joint_vjp),

@@ -3,8 +3,11 @@
 Used only when grad mode is on and a CUDA tensor input requires grad; every other call takes the value-only path.
 The backward passes are the library's derivative entry points (include/abrb.h):
 
-* dynamics: ``J^T g`` with the ``(B, n, n)`` derivatives of ``abrb_{forward,inverse}_dynamics_derivatives_*``;
-* ``simulate``: ``abrb_plant_rollout_vjp_*``, the adjoint recursion over the recorded states (DESIGN.md S3.6).
+* dynamics: ``J^T g`` with the ``(B, n, n)`` derivatives of ``abrb_{forward,inverse}_dynamics_derivatives_*``; the
+  link inertias ``theta`` through the regressor ``Y`` (``inverse_dynamics_regressor``): ``sum_b Y_b^T g_b`` for the
+  inverse dynamics, ``-sum_b Y_b^T M_b^-1 g_b`` (``Y`` at the computed ``ddq``) for the forward dynamics;
+* ``simulate``: ``abrb_plant_rollout_vjp_*``, the adjoint recursion over the recorded states (DESIGN.md S3.6), then
+  ``abrb_plant_rollout_theta_vjp_*`` for ``theta`` (DESIGN.md S3.8).
 
 The Functions are once-differentiable: a gradient of a gradient raises.
 """
@@ -45,28 +48,38 @@ def _ptr(t):
 
 class _Dynamics(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rc, kind, q, dq, x):
+    def forward(ctx, rc, kind, q, dq, x, theta):
         ctx.rc, ctx.kind = rc, kind
-        ctx.save_for_backward(q, dq, x)
-        return (rc.forward_dynamics if kind == 0 else rc.inverse_dynamics)(q, dq, x)
+        out = (rc.forward_dynamics if kind == 0 else rc.inverse_dynamics)(q, dq, x)
+        ctx.save_for_backward(q, dq, x, out if theta is not None else None, theta)
+        return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        q, dq, x = ctx.saved_tensors
-        d_q, d_dq, d_x = ctx.rc._derivatives(q, dq, x, ctx.kind, want_in=ctx.needs_input_grad[4])
+        q, dq, x, out, theta = ctx.saved_tensors
         g = g.contiguous()
+        gq = gdq = gx = gth = None
+        if any(ctx.needs_input_grad[2:5]):
+            d_q, d_dq, d_x = ctx.rc._derivatives(q, dq, x, ctx.kind, want_in=ctx.needs_input_grad[4])
 
-        def vjp(d, need):
-            return torch.bmm(g[:, None, :], d)[:, 0] if need else None
+            def vjp(d, need):
+                return torch.bmm(g[:, None, :], d)[:, 0] if need else None
 
-        return (None, None, vjp(d_q, ctx.needs_input_grad[2]), vjp(d_dq, ctx.needs_input_grad[3]),
-                vjp(d_x, ctx.needs_input_grad[4]))
+            gq, gdq, gx = (vjp(d, ctx.needs_input_grad[i]) for d, i in ((d_q, 2), (d_dq, 3), (d_x, 4)))
+        if ctx.needs_input_grad[5]:
+            if ctx.kind == 1:  # u = Y(q, dq, ddq) theta
+                w, Y = g, ctx.rc.inverse_dynamics_regressor(q, dq, x)
+            else:  # at fixed u, d ddq / d theta = -M^-1 Y(q, dq, ddq)
+                L = torch.linalg.cholesky(ctx.rc.eval(q, want=("M",))["M"])
+                w, Y = -torch.cholesky_solve(g[:, :, None], L)[:, :, 0], ctx.rc.inverse_dynamics_regressor(q, dq, out)
+            gth = torch.sum(torch.bmm(w[:, None, :], Y)[:, 0], 0).to(theta.dtype)
+        return None, None, gq, gdq, gx, gth
 
 
-def dynamics(rc, kind, q, dq, x):
+def dynamics(rc, kind, q, dq, x, theta=None):
     n = rc.N_JOINTS
-    ref = _ref_tensor(q, dq, x)
+    ref = _ref_tensor(q, dq, x, theta)
     dtype = q.dtype if isinstance(q, torch.Tensor) else ref.dtype
     ref = torch.empty((), dtype=dtype, device=ref.device)
     qa, dqa, xa = (_like(a, ref, w) for a, w in ((q, "q"), (dq, "dq"), (x, "u" if kind == 0 else "ddq")))
@@ -75,13 +88,22 @@ def dynamics(rc, kind, q, dq, x):
         if tuple(a.shape) != tuple(qa.shape) or a.shape[-1] != n or a.dim() not in (1, 2):
             raise ValueError(f"{w} must have the shape of q, ({n},) or (B, {n}), got {tuple(a.shape)}")
     qa, dqa, xa = (a.reshape(-1, n).contiguous() for a in (qa, dqa, xa))
-    out = _Dynamics.apply(rc, kind, qa, dqa, xa)
+    out = _Dynamics.apply(rc, kind, qa, dqa, xa, _grad_theta(theta, ref))
     return out[0] if single else out
+
+
+def _grad_theta(theta, ref):
+    """``theta`` when it takes part in the graph (a tensor that requires grad, on the inputs' device), else None"""
+    if not (isinstance(theta, torch.Tensor) and theta.requires_grad):
+        return None
+    if theta.device != ref.device:
+        raise ValueError(f"theta is on {theta.device}, the other inputs on {ref.device}")
+    return theta
 
 
 class _Simulate(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, rc, opts, q0, dq0, u, path):
+    def forward(ctx, rc, opts, q0, dq0, u, path, theta):
         ctx.set_materialize_grads(False)
         rec = opts["record"]
         inner = tuple(k for k in ("q", "dq", "u", "x") if k in rec or k in ("q", "dq"))
@@ -89,13 +111,13 @@ class _Simulate(torch.autograd.Function):
                                           compensate_gravity=opts["compensate_gravity"], ref_frame=opts["ref_frame"],
                                           xyz_offset=opts["xyz_offset"], record=inner)
         ctx.rc, ctx.opts = rc, opts
-        ctx.save_for_backward(q0, dq0, u, path, traj["q"], traj["dq"])
+        ctx.save_for_backward(q0, dq0, u, path, traj["q"], traj["dq"], theta)
         return (qf, dqf, cost) + tuple(traj[k] for k in rec)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g_qf, g_dqf, g_cost, *g_rec):
-        q0, dq0, u, path, q_traj, dq_traj = ctx.saved_tensors
+        q0, dq0, u, path, q_traj, dq_traj, theta = ctx.saved_tensors
         rc, opts = ctx.rc, ctx.opts
         B, n = q0.shape
         S = u.shape[0]
@@ -117,14 +139,24 @@ class _Simulate(torch.autograd.Function):
                           0 if path is None or path.dim() == 2 else 6, int(S), float(opts["dt"]),
                           float(opts["effort_weight"]), _ptr(q_traj), _ptr(dq_traj), *[_ptr(t) for t in cot],
                           gu.data_ptr(), gq0.data_ptr(), gdq0.data_ptr(), B, _stream(q0)))
+        gth = None
+        if ctx.needs_input_grad[6]:
+            gth = torch.empty((B, 6 * n), dtype=q0.dtype, device=q0.device)
+            fn = L.abrb_plant_rollout_theta_vjp_f32 if q0.dtype == torch.float32 else L.abrb_plant_rollout_theta_vjp_f64
+            with torch.cuda.device(q0.device):
+                _lib.check(fn(rc.handle, q0.data_ptr(), dq0.data_ptr(), _ptr(u), 0 if u.dim() == 2 else n,
+                              1 if opts["compensate_gravity"] else 0, int(S), float(opts["effort_weight"]),
+                              _ptr(q_traj), _ptr(dq_traj), gu.data_ptr(), _ptr(cot[0]), _ptr(cot[5]), gth.data_ptr(),
+                              B, _stream(q0)))
+            gth = torch.sum(gth, 0).to(theta.dtype)
         if u.dim() == 2:
             gu = gu.sum(1)
-        return None, None, gq0, gdq0, gu, None
+        return None, None, gq0, gdq0, gu, None, gth
 
 
-def simulate(rc, q, dq, u, dt, path, effort_weight, compensate_gravity, ref_frame, xyz_offset, record):
+def simulate(rc, q, dq, u, dt, path, effort_weight, compensate_gravity, ref_frame, xyz_offset, record, theta=None):
     n = rc.N_JOINTS
-    ref = _ref_tensor(q, dq, u)
+    ref = _ref_tensor(q, dq, u, theta)
     dtype = q.dtype if isinstance(q, torch.Tensor) else ref.dtype
     ref = torch.empty((), dtype=dtype, device=ref.device)
     qa, dqa = _like(q, ref, "q"), _like(dq, ref, "dq")
@@ -139,7 +171,7 @@ def simulate(rc, q, dq, u, dt, path, effort_weight, compensate_gravity, ref_fram
             raise ValueError(f"simulate can record 'q', 'dq', 'u' and 'x', not {k!r}")
     opts = dict(dt=dt, effort_weight=effort_weight, compensate_gravity=compensate_gravity, ref_frame=ref_frame,
                 xyz_offset=xyz_offset, record=tuple(record))
-    out = _Simulate.apply(rc, opts, qa, dqa, ua, pa)
+    out = _Simulate.apply(rc, opts, qa, dqa, ua, pa, _grad_theta(theta, ref))
     qf, dqf, cost = out[:3]
     traj = dict(zip(opts["record"], out[3:]))
     if single:

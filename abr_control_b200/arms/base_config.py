@@ -298,26 +298,43 @@ class BaseConfig:
             d = [t[0] for t in d]
         return tuple(d) if want_in else (d[0], d[1], None)
 
-    def forward_dynamics(self, q, dq, u):
+    def _with_theta(self, theta):
+        """The model with ``link_inertia[1:] = theta`` (``(6n,)``: a NumPy array or a float32/float64 CUDA tensor, read
+        back to the host once: a device synchronisation), for the ``theta`` argument of the plant's methods."""
+        if _is_torch(theta) and (not theta.is_cuda or theta.dtype not in (torch.float32, torch.float64)):
+            raise ValueError("theta must be a NumPy array or a float32/float64 CUDA tensor")
+        return self.with_link_inertia(theta)
+
+    def forward_dynamics(self, q, dq, u, theta=None):
         """Joint accelerations under the torque ``u``: ``ddq = M(q)^-1 (u + g(q) - C(q, dq) dq)``, the plant of the
         rollouts (``g`` is the gravity force the controllers subtract, so ``u = -g`` holds the arm still).
         ``q, dq, u`` are ``(n,)`` or ``(B, n)``; CUDA tensors in -> CUDA tensors out, NumPy in -> NumPy out.
-        Differentiable (``torch.autograd``, first order) when grad mode is on and a CUDA tensor input requires grad."""
-        if torch is not None and _is_torch_grad(q, dq, u):
+        Differentiable (``torch.autograd``, first order) when grad mode is on and a CUDA tensor input requires grad.
+
+        ``theta`` (``(6n,)``, see ``inertial_parameters``): evaluate with ``link_inertia[1:] = theta``, exactly as
+        ``with_link_inertia(theta).forward_dynamics(q, dq, u)`` (a tensor ``theta`` is read back to the host once per
+        call to build that model, a device synchronisation).  A CUDA ``theta`` that requires grad is differentiable
+        too: at fixed ``u``, ``Y(q, dq, ddq) theta = u`` gives ``d ddq / d theta = -M^-1 Y(q, dq, ddq)``, so
+        ``theta.grad = -sum_b Y(q_b, dq_b, ddq_b)^T M_b^-1 g_b`` for the output cotangent ``g`` (``Y``:
+        ``inverse_dynamics_regressor``)."""
+        rc = self if theta is None else self._with_theta(theta)
+        if torch is not None and _is_torch_grad(q, dq, u, theta):
             from . import _autograd
 
-            return _autograd.dynamics(self, 0, q, dq, u)
-        return self._dynamics(q, dq, u, "u", ("abrb_forward_dynamics_f64", "abrb_forward_dynamics_f32"))
+            return _autograd.dynamics(rc, 0, q, dq, u, theta)
+        return rc._dynamics(q, dq, u, "u", ("abrb_forward_dynamics_f64", "abrb_forward_dynamics_f32"))
 
-    def inverse_dynamics(self, q, dq, ddq):
+    def inverse_dynamics(self, q, dq, ddq, theta=None):
         """Torque that produces ``ddq``: ``u = M(q) ddq + C(q, dq) dq - g(q)`` (the inverse of ``forward_dynamics``),
         e.g. the feedforward torque of a planned joint trajectory.  Shapes and types as ``forward_dynamics``; likewise
-        differentiable."""
-        if torch is not None and _is_torch_grad(q, dq, ddq):
+        differentiable.  ``theta`` as in ``forward_dynamics``; ``u = Y(q, dq, ddq) theta`` is linear in it, so
+        ``theta.grad = sum_b Y(q_b, dq_b, ddq_b)^T g_b``."""
+        rc = self if theta is None else self._with_theta(theta)
+        if torch is not None and _is_torch_grad(q, dq, ddq, theta):
             from . import _autograd
 
-            return _autograd.dynamics(self, 1, q, dq, ddq)
-        return self._dynamics(q, dq, ddq, "ddq", ("abrb_inverse_dynamics_f64", "abrb_inverse_dynamics_f32"))
+            return _autograd.dynamics(rc, 1, q, dq, ddq, theta)
+        return rc._dynamics(q, dq, ddq, "ddq", ("abrb_inverse_dynamics_f64", "abrb_inverse_dynamics_f32"))
 
     # ------------------------------------------------------------------ inertial parameters
     def inverse_dynamics_regressor(self, q, dq, ddq):
@@ -421,7 +438,7 @@ class BaseConfig:
         return self._derivatives(q, dq, ddq, 1)
 
     def simulate(self, q, dq, u, dt=1e-3, path=None, effort_weight=0.0, compensate_gravity=False, ref_frame="EE",
-                 xyz_offset=None, record=("q", "dq", "u", "x")):
+                 xyz_offset=None, record=("q", "dq", "u", "x"), theta=None):
         """Open-loop rollout of the plant under the torque sequence ``u`` on the GPU (abrb_plant_rollout_*).  For each
         step ``t = 0 .. S-1``, with the semi-implicit Euler step of the reference (arms/twojoint/arm_sim.py:131-132)::
 
@@ -452,16 +469,54 @@ class BaseConfig:
         tensor that requires grad: gradients reach ``u`` (summed over trajectories for a shared ``(S, n)`` sequence),
         ``q`` and ``dq`` from the cost, the final state and every returned record, through the adjoint recursion of
         ``abrb_plant_rollout_vjp_*``.  The path, ``dt`` and ``effort_weight`` are constants; a path that requires
-        grad raises ``NotImplementedError``."""
+        grad raises ``NotImplementedError``.
+
+        ``theta`` (``(6n,)``, see ``inertial_parameters``): roll out the plant with ``link_inertia[1:] = theta``; values
+        and records are those of ``with_link_inertia(theta).simulate(...)`` (a tensor ``theta`` is read back to the
+        host once per call to build that model, a device synchronisation).  A CUDA ``theta`` that requires grad gets
+        its gradient too (DESIGN.md S3.8, ``abrb_plant_rollout_theta_vjp_*`` after the adjoint recursion): with
+        ``(q_t, dq_t)`` the state before step t, ``tau_t`` its applied torque, ``ddq_t = M^-1 (tau_t + g - C dq_t)``,
+        ``gu_t`` the per-trajectory torque cotangent, ``gc_b`` the cost cotangent and ``gr_t`` that of
+        ``traj["u"][t]``::
+
+            w_t        = gu_t - 2 effort_weight gc_b tau_t - gr_t         (the part of gu_t that flows through ddq_t)
+            theta.grad = sum_b sum_t [ -Y(q_t, dq_t, ddq_t)^T w_t + c_g Y(q_t, 0, 0)^T gu_t ]
+
+        with ``c_g = 1`` under ``compensate_gravity`` (then ``tau = u + Y(q, 0, 0) theta``) and 0 without.  The
+        control point, and so the path term of the cost, does not depend on ``theta``.
+
+        Output-error identification fits ``theta`` so that the plant replays a recorded track, with no ``ddq`` (nor
+        any differentiated measurement) needed.  Cut the recorded positions ``q_rec`` (``(T + 1, n)``) and applied
+        torques ``u_rec`` (``(T, n)``) into ``B`` windows of ``S`` steps that start at recorded states (``dq`` at a
+        window start from the record, or a free parameter), replay the recorded torques without compensation and
+        compare positions::
+
+            q0, dq0 = q_rec[starts], dq_rec[starts]                               # (B, n) window starts
+            u = torch.stack([u_rec[s:s + S] for s in starts], 1)                  # (S, B, n) recorded torques
+            target = torch.stack([q_rec[s + 1:s + S + 1] for s in starts], 1)     # (S, B, n)
+            theta = torch.tensor(rc.inertial_parameters(), device="cuda", requires_grad=True)
+
+            def loss():
+                _, _, traj, _ = rc.simulate(q0, dq0, u, dt=dt, compensate_gravity=False, record=("q",), theta=theta)
+                return (traj["q"] - target).pow(2).sum()
+
+        and minimise ``loss`` over ``theta`` (e.g. ``torch.optim.LBFGS``; for a link's three tied masses write
+        ``theta = T @ phi`` with ``arms._ident.tie_matrix(n)`` and optimise ``phi``).  Short windows keep the problem
+        well conditioned; directions of ``theta`` the motion does not excite stay where they start."""
         from ..controllers import _batch
 
+        rc = self if theta is None else self._with_theta(theta)
         if torch is not None and _is_torch(path) and path.requires_grad and torch.is_grad_enabled():
             raise NotImplementedError("simulate is not differentiable with respect to the path")
-        if torch is not None and _is_torch_grad(q, dq, u):
+        if torch is not None and _is_torch_grad(q, dq, u, theta):
             from . import _autograd
 
-            return _autograd.simulate(self, q, dq, u, dt, path, effort_weight, compensate_gravity, ref_frame,
-                                      xyz_offset, record)
+            return _autograd.simulate(rc, q, dq, u, dt, path, effort_weight, compensate_gravity, ref_frame,
+                                      xyz_offset, record, theta)
+        if rc is not self:
+            return rc.simulate(q, dq, u, dt=dt, path=path, effort_weight=effort_weight,
+                               compensate_gravity=compensate_gravity, ref_frame=ref_frame, xyz_offset=xyz_offset,
+                               record=record)
         qa, dqa, single, kind, f32 = self._on_device(q, dq)
         if kind == "torch":
             qa, dqa = qa.clone(), dqa.clone()

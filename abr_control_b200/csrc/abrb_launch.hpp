@@ -200,6 +200,22 @@ struct PlantVjpCall {
   cudaStream_t stream;
 };
 
+// abrb_plant_rollout_theta_vjp_*: the rollout's torques and recorded states, the torque cotangents gu of
+// abrb_plant_rollout_vjp_* and the cost and torque-record cotangents (nullptr: zero) -> g_theta (B, 6n)
+struct ThetaVjpCall {
+  const void *q0, *dq0, *u;
+  int u_stride;
+  int compensate_gravity;
+  int steps;
+  double effort_weight;
+  const void *q_traj, *dq_traj, *gu, *g_cost, *g_u_traj;
+  void *g_theta;
+  int64_t B;
+  const double *gravity;  // host, 6 values (the model's)
+  bool f32;
+  cudaStream_t stream;
+};
+
 // abrb_joint_rollout_path_vjp_*: the Joint rollout's arguments, its recorded states and the cotangents of its outputs
 // (each nullptr or device) -> the cotangents of the path, the path velocity and the gains (each nullptr when not
 // wanted; per trajectory), q0 and dq0
@@ -235,6 +251,7 @@ template <int N> int launch_regressor(const ChainHost &h, const RegressorCall &c
 template <int N> int launch_ctrl_rollout(const ChainHost &h, const CtrlRolloutCall &c);
 template <int N> int launch_dyn_jac(const ChainHost &h, const DynJacCall &c);
 template <int N> int launch_plant_vjp(const ChainHost &h, const PlantVjpCall &c);
+template <int N> int launch_theta_vjp(const ChainHost &h, const ThetaVjpCall &c);
 template <int N> int launch_joint_vjp(const ChainHost &h, const JointVjpCall &c);
 
 // Path planner (abrb_path_*): independent of the joint count, compiled in the ABRB_N == 1 unit only.  Device arrays.

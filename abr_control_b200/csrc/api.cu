@@ -1406,6 +1406,62 @@ int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *
                            gu, gq0, gdq0, B, stream, true);
 }
 
+static int plant_rollout_theta_vjp(const abrb_model *m, const void *q0, const void *dq0, const void *u, int u_stride,
+                                   int compensate_gravity, int steps, double effort_weight, const void *q_traj,
+                                   const void *dq_traj, const void *gu, const void *g_cost, const void *g_u_traj,
+                                   void *g_theta, int64_t B, void *stream, bool f32) {
+  const char *who = "abrb_plant_rollout_theta_vjp";
+  const std::string w(who);
+  if (!m) return fail(ABRB_EINVAL, w + ": NULL model");
+  if (B < 0) return fail(ABRB_EINVAL, w + ": B < 0");
+  if (steps < 0) return fail(ABRB_EINVAL, w + ": steps < 0");
+  const int n = m->host.n;
+  if (u_stride != 0 && u_stride != n) return fail(ABRB_EINVAL, w + ": u_stride must be 0 or n_joints");
+  if (!std::isfinite(effort_weight) || effort_weight < 0.0)
+    return fail(ABRB_EINVAL, w + ": effort_weight must be finite and >= 0");
+  if (B == 0) return ABRB_OK;
+  if (!q0) return fail(ABRB_EINVAL, w + ": NULL q0");
+  if (!dq0) return fail(ABRB_EINVAL, w + ": NULL dq0");
+  if (!g_theta) return fail(ABRB_EINVAL, w + ": NULL g_theta");
+  if (steps > 0) {
+    if (!u) return fail(ABRB_EINVAL, w + ": NULL u");
+    if (!q_traj) return fail(ABRB_EINVAL, w + ": NULL q_traj");
+    if (!dq_traj) return fail(ABRB_EINVAL, w + ": NULL dq_traj");
+    if (!gu) return fail(ABRB_EINVAL, w + ": NULL gu");
+  }
+  const void *ptrs[] = {q0, dq0, u, q_traj, dq_traj, gu, g_cost, g_u_traj, g_theta};
+  const char *names[] = {"q0", "dq0", "u", "q_traj", "dq_traj", "gu", "g_cost", "g_u_traj", "g_theta"};
+  for (int i = 0; i < 9; ++i)
+    if (ptrs[i] && !aligned_elem(ptrs[i], f32)) return fail(ABRB_EINVAL, w + ": misaligned pointer (" + names[i] + ")");
+  int rc = ensure_device();
+  if (rc) return rc;
+  ThetaVjpCall k{q0, dq0, u, u_stride, compensate_gravity, steps, effort_weight, q_traj, dq_traj, gu, g_cost, g_u_traj,
+                 g_theta, B, m->desc.gravity, f32, (cudaStream_t)stream};
+  int e = cudaErrorInvalidValue;
+  switch (n) {
+#define X(j) case j: e = launch_theta_vjp<j>(m->host, k); break;
+    ABRB_EACH_N(X)
+#undef X
+  }
+  return e ? cuda_fail(e, who) : ABRB_OK;
+}
+
+int abrb_plant_rollout_theta_vjp_f64(const abrb_model *m, const double *q0, const double *dq0, const double *u,
+                                     int u_stride, int compensate_gravity, int steps, double effort_weight,
+                                     const double *q_traj, const double *dq_traj, const double *gu,
+                                     const double *g_cost, const double *g_u_traj, double *g_theta, int64_t B,
+                                     void *stream) {
+  return plant_rollout_theta_vjp(m, q0, dq0, u, u_stride, compensate_gravity, steps, effort_weight, q_traj, dq_traj,
+                                 gu, g_cost, g_u_traj, g_theta, B, stream, false);
+}
+int abrb_plant_rollout_theta_vjp_f32(const abrb_model *m, const float *q0, const float *dq0, const float *u,
+                                     int u_stride, int compensate_gravity, int steps, double effort_weight,
+                                     const float *q_traj, const float *dq_traj, const float *gu, const float *g_cost,
+                                     const float *g_u_traj, float *g_theta, int64_t B, void *stream) {
+  return plant_rollout_theta_vjp(m, q0, dq0, u, u_stride, compensate_gravity, steps, effort_weight, q_traj, dq_traj,
+                                 gu, g_cost, g_u_traj, g_theta, B, stream, true);
+}
+
 static int joint_rollout_vjp(const abrb_model *m, JointVjpCall k) {
   const char *who = "abrb_joint_rollout_path_vjp";
   const std::string w(who);

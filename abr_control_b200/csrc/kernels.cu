@@ -18,6 +18,7 @@
 #include "abrb_path.cuh"
 #include "abrb_rbd.cuh"
 #include "abrb_regress.cuh"
+#include "abrb_theta.cuh"
 
 #ifndef ABRB_N
 #error "compile with -DABRB_N=<joint count>"
@@ -945,6 +946,58 @@ plant_vjp_kernel(const __grid_constant__ ChainK<Dual<T>, N> P, const __grid_cons
   }
 }
 
+template <typename T>
+struct ThetaVjpArgs {
+  const T *q0, *dq0, *u, *q_traj, *dq_traj, *gu, *g_cost, *g_u_traj;
+  T *g_theta;  // (B, 6N)
+  int64_t B;
+  int u_stride, steps, comp_g;
+  T effort;
+  T gravity[6];
+};
+
+// abrb_plant_rollout_theta_vjp_*: one warp per trajectory.  Lane i sums theta_vjp_state over the steps t = i, i + 32,
+// ... in order; the 32 partial sums are then combined by the same xor butterfly in every warp and lane 0 stores the
+// row.  So a trajectory's row depends on its own data only: bit-identical between runs and under permutation.
+template <typename T, int N, bool ORTHO>
+__global__ void __launch_bounds__(kBlock)
+theta_vjp_kernel(const __grid_constant__ ChainK<T, N> P, const __grid_constant__ ThetaVjpArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  typedef KinSel<T, N, ORTHO> KS;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  typename KS::type K;
+  KS::bind(K, reinterpret_cast<T *>(smem_raw) + warp * 32 * KS::kSlots, lane);
+  for (int64_t b = (int64_t)blockIdx.x * kWarps + warp; b < a.B; b += (int64_t)gridDim.x * kWarps) {
+    const T ec = a.g_cost != nullptr ? T(2) * a.effort * a.g_cost[b] : T(0);
+    T acc[6 * N];
+#pragma unroll
+    for (int p = 0; p < 6 * N; ++p) acc[p] = T(0);
+    for (int t = lane; t < a.steps; t += 32) {
+      const int64_t row = (int64_t)t * a.B + b;
+      const T *qs = t > 0 ? a.q_traj + (row - a.B) * N : a.q0 + b * N;
+      const T *dqs = t > 0 ? a.dq_traj + (row - a.B) * N : a.dq0 + b * N;
+      const T *ut = torque_row<T, N>(a.u, a.u_stride, t, a.B, b);
+      T q[N], dq[N], ur[N], gu[N], gt[N];
+#pragma unroll
+      for (int k = 0; k < N; ++k) {
+        q[k] = qs[k];
+        dq[k] = dqs[k];
+        ur[k] = ut[k];
+        gu[k] = a.gu[row * N + k];
+        gt[k] = a.g_u_traj != nullptr ? a.g_u_traj[row * N + k] : T(0);
+      }
+      theta_vjp_state<T, N>(P, a.gravity, q, dq, ur, a.comp_g != 0, gu, ec, gt, acc, K);
+    }
+#pragma unroll
+    for (int p = 0; p < 6 * N; ++p) {
+      T v = acc[p];
+#pragma unroll
+      for (int s = 16; s > 0; s >>= 1) v += __shfl_xor_sync(0xffffffffu, v, s);
+      if (lane == 0) a.g_theta[b * 6 * N + p] = v;
+    }
+  }
+}
+
 // The Joint closed loop's vector-Jacobian product has 4N + 2 working lanes (joint_vjp_lane): its dual kinematic
 // scratch is one column per working lane, (4N + 2) x KinSlots per warp, in CTAs of DualBlock<ORTHO> threads (UR5,
 // orthonormal: 22.5 KB a warp; a general 7-joint chain: 70.5 KB a warp).
@@ -1592,6 +1645,42 @@ int plant_vjp_go(const ChainHost &h, const PlantVjpCall &c) {
   kern<<<(unsigned)(blocks < cap ? blocks : cap), DualBlock<ORTHO>::value, smem, c.stream>>>(P, a);
   count_launch();
   return (int)cudaGetLastError();
+}
+
+template <typename T, int N, bool ORTHO>
+int theta_vjp_go(const ChainHost &h, const ThetaVjpCall &c) {
+  ChainK<T, N> P;
+  fill_chain<T, N>(h, P);
+  ThetaVjpArgs<T> a;
+  a.q0 = static_cast<const T *>(c.q0);
+  a.dq0 = static_cast<const T *>(c.dq0);
+  a.u = static_cast<const T *>(c.u);
+  a.q_traj = static_cast<const T *>(c.q_traj);
+  a.dq_traj = static_cast<const T *>(c.dq_traj);
+  a.gu = static_cast<const T *>(c.gu);
+  a.g_cost = static_cast<const T *>(c.g_cost);
+  a.g_u_traj = static_cast<const T *>(c.g_u_traj);
+  a.g_theta = static_cast<T *>(c.g_theta);
+  a.B = c.B;
+  a.u_stride = c.u_stride;
+  a.steps = c.steps;
+  a.comp_g = c.compensate_gravity;
+  a.effort = T(c.effort_weight);
+  for (int i = 0; i < 6; ++i) a.gravity[i] = T(c.gravity[i]);
+  const size_t smem = (size_t)kBlock * KinSel<T, N, ORTHO>::kSlots * sizeof(T);
+  auto kern = theta_vjp_kernel<T, N, ORTHO>;
+  cudaError_t e = set_smem(kern, smem);
+  if (e != cudaSuccess) return (int)e;
+  const int64_t blocks = (c.B + kWarps - 1) / kWarps, cap = (int64_t)num_sms() * 16;
+  kern<<<(unsigned)(blocks < cap ? blocks : cap), kBlock, smem, c.stream>>>(P, a);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+template <>
+int launch_theta_vjp<ABRB_N>(const ChainHost &h, const ThetaVjpCall &c) {
+  if (c.f32) return h.ortho ? theta_vjp_go<float, ABRB_N, true>(h, c) : theta_vjp_go<float, ABRB_N, false>(h, c);
+  return h.ortho ? theta_vjp_go<double, ABRB_N, true>(h, c) : theta_vjp_go<double, ABRB_N, false>(h, c);
 }
 
 template <typename T, int N, bool ORTHO>

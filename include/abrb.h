@@ -436,6 +436,31 @@ int abrb_plant_rollout_vjp_f32(const abrb_model *m, int frame_id, const double *
                                const float *g_u_traj, const float *g_x_traj, float *gu, float *gq0, float *gdq0,
                                int64_t B, void *stream);
 
+/* Gradient of abrb_plant_rollout_* with respect to the link inertias theta = link_inertia[1:] flattened (theta[6 (l-1)
+ * + c], as abrb_inverse_dynamics_regressor_*).  Given the rollout's start state, torques and recorded states (q_traj,
+ * dq_traj: (steps, B, n)), the torque cotangents gu (steps, B, n) that abrb_plant_rollout_vjp_* wrote for the same
+ * output cotangents, and the cotangents g_cost (B) and g_u_traj (steps, B, n) of the cost and of the recorded torques
+ * (each NULL: zero), writes
+ *     g_theta (B, 6n) = sum_t [ -Y(q_t, dq_t, ddq_t)^T w_t + c_g Y(q_t, 0, 0)^T gu_t ],
+ *     w_t = gu_t - 2 effort_weight g_cost tau_t - g_u_traj[t]
+ * per trajectory (the gradient of the shared model is the sum over B).  (q_t, dq_t) is the state before step t, tau_t
+ * its applied torque, ddq_t = M^-1 (tau_t + g - C dq_t) recomputed from them, c_g = 1 with compensate_gravity and 0
+ * without.  The frame, offset and path do not depend on theta; dt enters through gu.  steps == 0 writes zeros, B == 0
+ * does nothing.  No atomics: rows are bit-identical between runs and under a permutation of the trajectories.
+ * Argument errors (before any device work) as abrb_plant_rollout_vjp_*: ABRB_EINVAL for a NULL model, q0, dq0 or
+ * g_theta, (steps > 0) a NULL u, q_traj, dq_traj or gu, B < 0, steps < 0, u_stride not 0 or n, a negative or
+ * non-finite effort_weight, misaligned pointers.
+ * ------------------------------------------------------------------------------------------------- */
+int abrb_plant_rollout_theta_vjp_f64(const abrb_model *m, const double *q0, const double *dq0, const double *u,
+                                     int u_stride, int compensate_gravity, int steps, double effort_weight,
+                                     const double *q_traj, const double *dq_traj, const double *gu,
+                                     const double *g_cost, const double *g_u_traj, double *g_theta, int64_t B,
+                                     void *stream);
+int abrb_plant_rollout_theta_vjp_f32(const abrb_model *m, const float *q0, const float *dq0, const float *u,
+                                     int u_stride, int compensate_gravity, int steps, double effort_weight,
+                                     const float *q_traj, const float *dq_traj, const float *gu, const float *g_cost,
+                                     const float *g_u_traj, float *g_theta, int64_t B, void *stream);
+
 /* Vector-Jacobian product of abrb_joint_rollout_path_*: given the rollout's arguments (q0, dq0: the START state), the
  * states it recorded (q_traj, dq_traj: (steps, B, n), required when steps > 0) and cotangents of its outputs, each
  * NULL (zero) or as in abrb_plant_rollout_vjp_* (g_u_traj: of the recorded Joint torques u), writes
